@@ -1,12 +1,14 @@
 #!/usr/bin/env python
 """bench.py — decoded+aggregated rows/s of the fused scan/aggregate path (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W          # our arm (libogpu.so, sm_100a kernels)
+    python bench.py --gpus N --steps K --warmup W          # our arm (libogpu.so, sm_90a kernels)
     python bench.py --impl reference --gpus N ...          # reference arm: the CPU oracle on the host cores
+    python bench.py ... --dump-outputs DIR                 # also write the last timed step's answer as DIR/<name>.npy
 
-Workload (config.workload): BASELINE.json configs[1] — one TSM shard of 10k series x 1M points/series of float64
+Workload (config.workload): BASELINE.json configs[1] — one TSM shard of 5k series x 1M points/series of float64
 (G-hi distribution: 100 + U[0,1) with full mantissa tail -> Gorilla ~6 B/value), 1 s cadence, const-delta time pages,
-1000-row segments; SELECT sum, count (mean) and max GROUP BY time(1m), all series in one tagset.
+1000-row segments; SELECT sum, count (mean) and max GROUP BY time(1m), all series in one tagset.  5k series keep the
+30 GB of pages and the 31 GB lane-interleaved copy the fused kernel reads (DESIGN.md) inside one 80 GB H100.
 A "step" = one og_query_run over the whole HBM-resident shard (k_fused_fast over the lane-interleaved Gorilla streams, k_fused_raw for raw pages, edge stitch + tagset
 merge).  At N > 1 every rank holds its own shard (distinct seed; configs[3]) and a step ends with the NCCL
 cross-shard merge of the dense bucket arrays (weak scaling).
@@ -36,7 +38,7 @@ def parse():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--series", type=int, default=10_000)
+    ap.add_argument("--series", type=int, default=5_000)
     ap.add_argument("--rows", type=int, default=1_000_000)
     ap.add_argument("--dist", default="hi", choices=["hi", "lo"])
     ap.add_argument("--e2e-series", type=int, default=2000, help="series of the host-resident sample used by the e2e leg")
@@ -49,11 +51,32 @@ def parse():
     ap.add_argument("--nulls", type=int, default=0, help="mixed workload: null permille of every column (50 = the 5 %% variant)")
     ap.add_argument("--no-verify", action="store_true", help="skip the answer check after the timed loop")
     ap.add_argument("--verify-series", type=int, default=4, help="series sampled for the bitwise check against the oracle")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the dense result of the last step as DIR/<i>_<func>_<col>.npy and "
+                         "DIR/<i>_<func>_<col>_valid.npy (float64) so that two builds can be compared output for output")
+    a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be >= 1")
+    if a.dump_outputs and a.workload == "downsample":
+        ap.error("--dump-outputs covers the float and mixed workloads (the downsample pass returns encoded pages)")
+    return a
+
+
+def dump_dense(out_dir, d, calls):
+    """The dense interval record a caller of og_query_run receives, one file per array: values as float64 (counts and int sums
+    below 2^53 are exact), validity as float64 0/1, selector times (when the record carries them) as float64 ns after T0."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for k, (func, col) in enumerate(calls):
+        c, name = d["cols"][k], f"{k}_{func}_{col}"
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(c["values"]).astype(np.float64))
+        np.save(os.path.join(out_dir, f"{name}_valid.npy"), np.asarray(c["valid"]).astype(np.float64))
+        if c["times"] is not None:
+            np.save(os.path.join(out_dir, f"{name}_times.npy"), (np.asarray(c["times"]) - T0).astype(np.float64))
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe), in-process through NVML
+    """SM clock and throttle reasons sampled DURING the timed region, in-process through NVML
     (a background thread; og_query_run releases the GIL), falling back to one nvidia-smi query when NVML is missing."""
 
     def __init__(self, index):
@@ -92,14 +115,22 @@ class ClockSampler:
                 self._poll_once()
             sm = sorted(r[0] for r in self.rows)
             reasons = sorted({n for r in self.rows for bit, n in names.items() if r[2] & bit})
-            return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max((r[1] for r in self.rows), default=None),
-                    "reasons": reasons, "samples": len(sm), "source": "nvml"}
+            gpu, power = None, None
+            try:
+                gpu = self.nv.nvmlDeviceGetName(self.h)
+                gpu = gpu.decode() if isinstance(gpu, bytes) else gpu
+                power = self.nv.nvmlDeviceGetEnforcedPowerLimit(self.h) / 1000.0
+            except Exception:
+                pass
+            return {"gpu": gpu, "power_limit_w": power, "sm_mhz": sm[len(sm) // 2] if sm else None,
+                    "sm_max_mhz": max((r[1] for r in self.rows), default=None), "reasons": reasons, "samples": len(sm), "source": "nvml"}
         try:
-            out = subprocess.run(["nvidia-smi", f"--id={self.index}", "--query-gpu=clocks.sm,clocks.max.sm", "--format=csv,noheader,nounits"],
+            out = subprocess.run(["nvidia-smi", f"--id={self.index}", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader,nounits"],
                                  capture_output=True, text=True, timeout=10).stdout.split(",")
-            return {"sm_mhz": int(float(out[0])), "sm_max_mhz": int(float(out[1])), "reasons": [], "samples": 1, "source": "nvidia-smi after the region"}
+            return {"gpu": out[0].strip(), "power_limit_w": float(out[1]), "sm_mhz": int(float(out[2])), "sm_max_mhz": int(float(out[3])),
+                    "reasons": [], "samples": 1, "source": "nvidia-smi after the region"}
         except Exception:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvml and nvidia-smi unavailable"], "samples": 0}
+            return {"gpu": None, "power_limit_w": None, "sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvml and nvidia-smi unavailable"], "samples": 0}
 
     def _poll_once(self):
         self.stop_flag = True
@@ -110,27 +141,12 @@ class ClockSampler:
             pass
 
 
-def ncu_traffic(a):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel from the committed ncu --set full capture
-    (profiles/traffic.json); only valid for the workload it was captured on, else null."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        if a.workload == "mixed":
-            if a.series == 10000 and a.rows == 1000000 and a.nulls == 0:  # the mixed workload's own defaults (50k x 20k) are substituted for these
-                return t["k_fused_cols"]["dram_bytes_per_launch"]
-        elif a.series == 10000 and a.rows == 1000000 and a.dist == "hi":
-            return t["k_fused_il"]["dram_bytes_per_launch"]
-    except Exception:
-        pass
-    return None
-
-
 def measured_peak():
     try:
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measured peak"
 
 
 def workload_name(a):
@@ -148,8 +164,8 @@ def dist_const(L, a):
 # ---------------------------------------------------------------------------------------------------------------
 def host_threads():
     """Threads the CPU arm can really use: hardware threads visible to this process, capped by the container's CPU quota
-    (cgroup cpu.max) — on the graft B200 boxes nproc says 128 but the quota is 16 CPUs, and running 128 threads under a
-    16-CPU quota is slower than 16-32.  Returns (candidate thread counts, note)."""
+    (cgroup cpu.max) — in a container nproc can report every host thread (say 128) under a quota of 16 CPUs, and running
+    128 threads under a 16-CPU quota is slower than 16-32.  Returns (candidate thread counts, note)."""
     hw = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
     quota = None
     try:
@@ -414,6 +430,8 @@ def run_ours(a):
     dev_ms_max, wall_ms_max = t.tolist()
     total_rows = rows_t.item()
     value = total_rows * a.steps / (dev_ms_max / 1e3)
+    if a.dump_outputs and rank == 0:  # at N > 1 the dense arrays hold the cross-shard merge of the last step
+        dump_dense(a.dump_outputs, q.dense_host(), calls)
 
     # warm end-to-end: the shard stays resident in HBM (the deployment this library is built for: a shard is uploaded once and
     # queried many times); a step = og_query_run + draining og_query_next into host records
@@ -444,7 +462,7 @@ def run_ours(a):
     kernel_name = {3: "k_fused_il<SUM|COUNT|MAX, fold> (+ k_fused_segment for %d general segments)" % st["general_segments"],
                    2: "k_fused_il<SUM|COUNT|MAX> (+ k_fused_segment)", 1: "k_fused_segment", 0: "k_decode_tile+k_filter_tile+k_window_reduce"}[st["path"]]
     roofline = {"bound": "hbm", "kernel": kernel_name, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": ncu_traffic(a), "peak_source": peak_src, "algorithmic_bytes_per_launch": algo_bytes,
+                "peak_source": peak_src, "algorithmic_bytes_per_launch": algo_bytes,
                 "bytes_per_row": algo_bytes / max(1, st["rows_decoded"]), "kernel_ms": main_per_launch_ms,
                 "share_of_step": main_ms / max(1e-9, dev_ms if world == 1 else main_ms),
                 "interleaved_copy": {"build_ms_once_per_shard": st["il_build_ms"], "bytes": st["il_bytes"], "state": st["il_state"],
@@ -515,7 +533,7 @@ def run_ours(a):
         e2e = {"value": e_rows * e_steps / et.item(), "unit": "rows/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": max(d2h, d2h_full),
                "sample": f"{ns} series x {a.rows} rows per GPU per step (host-resident, pinned), og_shard_open + og_query_run + og_query_next",
                "resident": resident,
-               "sample_note": "2000 of the 10000 series per step: pinning and re-uploading the full 61 GB shard every step would take minutes; rates, not totals, are compared",
+               "sample_note": f"{ns} of the {a.series} series per step: pinning and re-uploading the full shard every step would take minutes; rates, not totals, are compared",
                "steps": e_steps, "phase_ms_per_step": {k: round(v / e_steps, 2) for k, v in phases.items()}, "ms_per_step": et.item() / e_steps * 1e3, "out_rows": out_rows}
         # the cold path is the host-to-device copy: og_shard_open is one blocking copy of the pages plus the directory
         open_s = phases.get("open", 0.0) / e_steps / 1e3
@@ -561,7 +579,7 @@ def run_ours(a):
                 "data": "synthetic", "impl": "ours",
                 "config": {"workload": workload_name(a), "shards": world, "rows_per_shard": int(info["n_rows"]), "segments_per_shard": int(info["n_segments"]),
                            "page_bytes_per_shard": int(info["page_bytes"]), "compressed_bytes_per_value": info["page_bytes"] / max(1, info["n_rows"]),
-                           "l2": "inputs (tens of GB per step) are far larger than the 126 MB L2; no explicit flush",
+                           "l2": "inputs (tens of GB per step) are far larger than the 50 MB L2 of an H100; no explicit flush",
                            "parallelism": f"shard-per-gpu x{world}" + (", og_query_allreduce: NCCL all-reduce(sum,count) + all-gather/fold(max) inside libogpu.so" if world > 1 else ""),
                            "timing": "CUDA events on the query stream (og_stats.kernel_ms + og_stats.merge_ms); max over ranks",
                            "merge_ms_per_step": merge_ms_total[0] / (max(a.warmup, 3) + a.steps) if world > 1 else 0.0,
@@ -588,7 +606,7 @@ def run_mixed(a):
     from opengemini_b200 import _lib as L
     torch.cuda.set_device(0)
     Shard.init(0)
-    series = a.series if a.series != 10_000 else 50_000
+    series = a.series if a.series != 5_000 else 50_000
     rows = a.rows if a.rows != 1_000_000 else 20_000
     cols = [(L.TYPE_INT, L.SYNTH_INT_WALK, a.nulls), (L.TYPE_FLOAT, L.SYNTH_F_LO, a.nulls), (L.TYPE_BOOL, L.SYNTH_BOOL, a.nulls)]
     sh = Shard.synth(series, rows, cols, t0=T0, dt=SEC, seed=4242)
@@ -605,6 +623,8 @@ def run_mixed(a):
         q.run(); st = q.stats()
         dev_ms += st["kernel_ms"]; main_ms += st["main_kernel_ms"]; launches += st["kernel_launches"]
     clocks = sampler.stop()
+    if a.dump_outputs:
+        dump_dense(a.dump_outputs, q.dense_host(), calls)
     # answer check on a slice: the first K series of the population, same seed, through the oracle
     verify = None
     if not a.no_verify:
@@ -628,9 +648,9 @@ def run_mixed(a):
             "config": {"workload": f"configs[2]: {series} series x {rows} rows, int64 (Simple8b) + float64 (Gorilla G-lo) + bool columns, {a.nulls / 10:.0f}% nulls, "
                                    "count(i), sum(i), sum(f), count(b) WHERE f > 1000 GROUP BY time(1m), one tagset", "rows": int(info["n_rows"]),
                        "page_bytes": int(info["page_bytes"]), "compressed_bytes_per_row": info["page_bytes"] / max(1, info["n_rows"]),
-                       "l2": "3 GB of pages per step: far larger than the 126 MB L2; no explicit flush"},
+                       "l2": "3 GB of pages per step: far larger than the 50 MB L2 of an H100; no explicit flush"},
             "clocks": clocks, "roofline": {"bound": "hbm", "kernel": "k_fused_cols" if st["path"] == 5 else "k_fused_multi", "achieved": algo / (k_ms / 1e3) / 1e9, "peak": peak, "unit": "GB/s",
-                                           "frac": algo / (k_ms / 1e3) / 1e9 / peak, "traffic": ncu_traffic(a) if st["path"] == 5 else None, "peak_source": peak_src, "algorithmic_bytes_per_launch": algo,
+                                           "frac": algo / (k_ms / 1e3) / 1e9 / peak, "peak_source": peak_src, "algorithmic_bytes_per_launch": algo,
                                            "kernel_ms": k_ms, "note": "instruction-bound: three codecs decoded per row by one thread; bytes per row are ~3"},
             "e2e": None, "cpu_baseline": None, "verify": verify, "gpu_launches": launches, "path": st["path"]}
     print(json.dumps(line), flush=True)
@@ -651,7 +671,7 @@ def run_downsample(a):
     from opengemini_b200.downsample import downsample
     torch.cuda.set_device(0)
     Shard.init(0)
-    series = a.series if a.series != 10_000 else 125
+    series = a.series if a.series != 5_000 else 125
     rows = a.rows
     sh = Shard.synth(series, rows, [(L.TYPE_FLOAT, L.SYNTH_F_HI if a.dist == "hi" else L.SYNTH_F_LO, 0)], t0=T0, dt=SEC, seed=99)
     info = sh.info()

@@ -1,5 +1,5 @@
 /*
- * ogpu.h — C ABI of libogpu.so: the B200-native scan/aggregate path behind openGemini's
+ * ogpu.h — C ABI of libogpu.so: the H100 (sm_90a) scan/aggregate path behind openGemini's
  * cursor seam.  Plain pointers and sizes only; no C++/torch types cross this boundary.
  *
  * What each entry point replaces in the reference (paths relative to the openGemini tree):

@@ -1,6 +1,6 @@
-"""opengemini_b200 — B200-native scan/aggregate path behind openGemini's cursor seam.
+"""opengemini_b200 — H100-native scan/aggregate path behind openGemini's cursor seam (the package keeps its original name).
 
-Product = libogpu.so (hand-written sm_100a CUDA behind the C ABI in include/ogpu.h).
+Product = libogpu.so (hand-written sm_90a CUDA behind the C ABI in include/ogpu.h).
 This package only holds the host-side bindings; aggregation and decoding never run on the CPU
 (the bindings only slice the records the library returns).
 """

@@ -122,7 +122,7 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                           "(nvcc, sm_100a). There is no CPU fallback for the scan/aggregate path.")
+                           "(nvcc, sm_90a). There is no CPU fallback for the scan/aggregate path.")
     L = C.CDLL(LIB_PATH)
     L.og_strerror.restype = C.c_char_p
     L.og_strerror.argtypes = [C.c_int]

@@ -166,7 +166,7 @@ OG_API const char *og_strerror(int st) {
     }
 }
 OG_API const char *og_last_error(void) { return g_err; }
-OG_API const char *og_version(void) { return "ogpu 0.2 (sm_100a)"; }
+OG_API const char *og_version(void) { return "ogpu 0.2 (sm_90a)"; }
 OG_API int og_release_cached_memory(void) {
     if (g_device < 0) return OG_OK;
     CU(cudaSetDevice(g_device));

@@ -1,5 +1,5 @@
 /*
- * decode.cuh — device-side page parsing and column block decoders (sm_100a).
+ * decode.cuh — device-side page parsing and column block decoders (sm_90a).
  *
  * One thread owns one page and walks it sequentially, handing each decoded value to an `emit(i, bits)` functor,
  * so the same decoders serve the materialise kernels (emit = store) and the fused aggregate kernels

@@ -265,7 +265,7 @@ __device__ __forceinline__ void cols_column(const DirP &d, const QueryP &q, cons
 }
 
 #ifndef OG_COLS_MINB
-#define OG_COLS_MINB 10 /* blocks/SM the register cap allows; measured at configs[2]: 4 -> 52, 5 -> 62, 6 -> 64, 8 -> 71, 10 -> 73, 12 -> 74 G rows/s; with the slimmer row loops 8 -> 85, 10 -> 87, 12 -> 86 */
+#define OG_COLS_MINB 8 /* blocks/SM the register cap allows; k_fused_cols at configs[2] on an H100 (400 W), ms per 10^9 rows: 8 -> 12.28, 10 -> 12.35-12.54, 12 -> 14.5 */
 #endif
 template <bool SIMPLE>
 __global__ void __launch_bounds__(128, SIMPLE ? OG_COLS_MINB : 4) k_fused_cols(DirP d, QueryP q, ChunkP ch) {

@@ -77,11 +77,11 @@ enum { SEG_GENERAL = 0, SEG_FAST = 1, SEG_RAWX = 2 }; /* static per-segment clas
 #define OG_IL_B 16u             /* rows per bulk copy (2 KB) */
 #endif
 #ifndef OG_IL_K
-#define OG_IL_K 10u             /* records per round.  Measured fraction of the HBM peak at configs[1] with boundary-aligned rounds:
-                                   8 -> 0.623, 10 -> 0.631, 12 -> 0.618 (before alignment: 8 -> 0.572, 10 -> 0.573, 12 -> 0.577, 14 -> 0.541, 16 -> 0.557) */
+#define OG_IL_K 10u             /* records per round.  k_fused_il at configs[1] on an H100 (400 W), ms: 8 -> 14.49-14.50,
+                                   10 -> 14.45-14.47, 12 -> 14.48-14.50 */
 #endif
 #ifndef OG_IL_UNROLL
-#define OG_IL_UNROLL 2 /* two pairs per loop trip: measured 1.4 % faster than the fully unrolled round (instruction cache) */
+#define OG_IL_UNROLL 2 /* two pairs per loop trip rather than the fully unrolled round, which is hard on the instruction cache */
 #endif
 #define OG_IL_NB (OG_IL_NW / OG_IL_B)
 #define OG_IL_ROWS (OG_IL_NW + 2u) /* + 2 mirror rows that repeat ring rows 0,1 so that three consecutive rows never wrap */

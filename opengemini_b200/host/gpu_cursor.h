@@ -19,7 +19,7 @@
  *     way aggregateCursor.SinkPlan does (aggregate_cursor.go:208-242).
  *   - Errors are values (Go `error`): every call that can fail returns an Error with code = the C-ABI status and the
  *     library's message.  A cursor is confined to one thread at a time (SURVEY §8b Threading).
- *   - There is no CPU path: if libogpu.so cannot bind a B200 every call fails with OG_E_CUDA.
+ *   - There is no CPU path: if libogpu.so cannot bind an H100 every call fails with OG_E_CUDA.
  */
 #pragma once
 #include <cstdint>

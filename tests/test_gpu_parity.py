@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the C ABI, against the CPU oracle.
+"""GPU parity tests (need an H100): the CUDA path, called through the C ABI, against the CPU oracle.
 
 Bar: bit-exact for everything, including float sums when the query asks for OG_Q_STRICT_ORDER — the kernels then keep
 the reference's summation order (left-to-right inside a record window, prev+curr across records, series order across

@@ -1,7 +1,7 @@
 """Parity at the sizes BASELINE.json names (not only at toy sizes):
 
 * configs[0]: 100 series x 10k float64 points, mean (sum, count) GROUP BY time(1m) — the reference's CPU-runnable case.
-* a 1/100 slice of configs[1]: 100 series x 10^6 points, G-hi and G-lo, sum/count/max GROUP BY time(1m), against the oracle on
+* a 1/50 slice of configs[1]: 100 of its 5000 series x 10^6 points, G-hi and G-lo, sum/count/max GROUP BY time(1m), against the oracle on
   the identical synthetic shard (same seed): strict order bitwise, folded order 1e-12 on float sums and bitwise on the rest,
   per-series grouping bitwise.
 """
