@@ -643,7 +643,7 @@ int build_plan(og_query *q) {
     uint32_t *d_grp_begin, *d_grp_series;
     if ((rc = salloc(q, &d_grp_begin, grp_begin.size()))) return rc;
     if ((rc = salloc(q, &d_grp_series, grp_series.size()))) return rc;
-    if ((rc = salloc(q, &q->d_err, 8))) return rc;
+    if ((rc = salloc(q, &q->d_err, 16))) return rc;
     CU(cudaMemcpyAsync(d_grp_begin, grp_begin.data(), grp_begin.size() * 4, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(d_grp_series, grp_series.data(), grp_series.size() * 4, cudaMemcpyHostToDevice, st));
     CU(cudaStreamSynchronize(st)); /* the host vectors die with this frame */
@@ -789,7 +789,7 @@ OG_API int og_query_run(og_query *q) {
     DirP dir = make_dir(s);
     uint32_t launches = 0, n_chunks = (s->n_series + q->chunk_series - 1) / q->chunk_series;
     while (q->main_ev.size() < 2 * (size_t)n_chunks) { cudaEvent_t e; CU(cudaEventCreate(&e)); q->main_ev.push_back(e); }
-    CU(cudaMemsetAsync(q->d_err, 0, 32, st));
+    CU(cudaMemsetAsync(q->d_err, 0, 64, st));
     CU(cudaEventRecord(q->ev0, st));
     const bool per_series = q->desc.group_mode == OG_GROUP_PER_SERIES;
     if (!per_series) { k_init_dense<<<(unsigned)((cells_dense + 255) / 256), 256, 0, st>>>(p, gp); launches++; } /* per-series: k_merge_per_series writes every cell */
@@ -873,9 +873,14 @@ OG_API int og_query_run(og_query *q) {
     CU(cudaEventRecord(q->ev1, st));
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(st));
-    int err[8];
-    CU(cudaMemcpy(err, q->d_err, 32, cudaMemcpyDeviceToHost));
-    if (getenv("OGPU_IL_STATS")) fprintf(stderr, "[ogpu] fused rounds: common %d rare %d (lanes not resident in %d, sit-outs %d)\n", err[4], err[5], err[6], err[7]);
+    int err[16];
+    CU(cudaMemcpy(err, q->d_err, 64, cudaMemcpyDeviceToHost));
+    if (getenv("OGPU_IL_STATS")) {
+        unsigned long long wait, life; /* warp cycles waiting for ring batches / over the warp's lifetime (OG_IL_STATS builds) */
+        memcpy(&wait, err + 8, 8); memcpy(&life, err + 10, 8);
+        fprintf(stderr, "[ogpu] fused rounds: common %d rare %d (lanes not resident in %d, sit-outs %d); warp cycles: %llu waiting for batches of %llu (%.1f %%)\n",
+                err[4], err[5], err[6], err[7], wait, life, life ? 100.0 * (double)wait / (double)life : 0.0);
+    }
     q->cells_dirty = err[2] != 0;
     if (err[0]) { set_error("segment %d failed to decode (device code %d)", err[1], err[0]); return map_dev_err(err[0]); }
     float ms = 0; cudaEventElapsedTime(&ms, q->ev0, q->ev1);

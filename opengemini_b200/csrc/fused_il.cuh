@@ -11,9 +11,12 @@
  *             their streams at nearly the same rate, which (a) bounds the padding to the group maximum at ~1 % instead of
  *             ~10 % and (b) lets the whole warp share one window of rows.
  *   staging   rows [f, f+NW) of the group live in a shared-memory ring; ONE lane refills it with cp.async.bulk (TMA, UBLKCP)
- *             in batches of OG_IL_B rows (1 KB contiguous in HBM and in shared memory) that complete on an mbarrier per
- *             batch slot.  No per-lane copies, no per-lane address arithmetic.  A lane whose next OG_IL_K records could
- *             touch rows that are not resident yet sits the round out (it only happens when lanes drift apart by more
+ *             in batches of OG_IL_B rows (2 KB contiguous in HBM and in shared memory) that complete on an mbarrier per
+ *             batch slot.  No per-lane copies, no per-lane address arithmetic.  Every line of the interleaved copy is read
+ *             exactly once, so the copies carry an L2::evict_first policy: they leave L2 first instead of ageing out with
+ *             normal priority (DESIGN.md "Staging" has the H100 numbers; an L2 prefetch of later batches ahead of the ring,
+ *             cp.async.bulk.prefetch.L2, measured slower than the hint alone at every depth tried).  A lane whose next
+ *             OG_IL_K records could touch rows that are not resident yet sits the round out (it only happens when lanes drift apart by more
  *             than ~30 rows, i.e. when binning could not match them).
  *   decode    stateless bit addressing: three LDS.32 at immediate row offsets + two funnel shifts give the 64 stream bits
  *             at bit position q.  q is kept so that the '10' (window reuse) record's payload lands in place:
@@ -77,8 +80,8 @@ enum { SEG_GENERAL = 0, SEG_FAST = 1, SEG_RAWX = 2 }; /* static per-segment clas
 #define OG_IL_B 16u             /* rows per bulk copy (2 KB) */
 #endif
 #ifndef OG_IL_K
-#define OG_IL_K 10u             /* records per round.  k_fused_il at configs[1] on an H100 (400 W), ms: 8 -> 14.49-14.50,
-                                   10 -> 14.45-14.47, 12 -> 14.48-14.50 */
+#define OG_IL_K 10u             /* records per round.  k_fused_il at configs[1] on an H100 (700 W), evict-first ring copies,
+                                   ms: 8 -> 11.73, 10 -> 11.74, 12 -> 11.77 (8 and 10 within 0.1 %) */
 #endif
 #ifndef OG_IL_UNROLL
 #define OG_IL_UNROLL 2 /* two pairs per loop trip rather than the fully unrolled round, which is hard on the instruction cache */
@@ -169,6 +172,10 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
     __shared__ __align__(8) uint64_t s_bar[WPB * NB];
     extern __shared__ __align__(8) uint8_t s_acc[]; /* FOLD: WPB x il_acc_bytes */
 
+#ifdef OG_IL_STATS
+    const long long st_clk0 = clock64();
+    long long st_wait = 0; /* cycles spent waiting for ring batches to land */
+#endif
     const uint32_t lane = threadIdx.x & 31;
     /* warp-uniform values are produced by warp reductions so that the compiler keeps them (and everything derived from them:
      * ring/barrier addresses, batch counters) in uniform registers — the bulk-copy instructions take uniform operands */
@@ -218,20 +225,23 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
     uint32_t hung = 0;                  /* warp-uniform watchdog code: 1 a batch never landed, 2 the round limit was hit */
     /* every lane calls issue(); one elected lane performs it.  The batch index goes through a warp reduction so that slot, ring,
      * barrier and source addresses are uniform-register arithmetic (the bulk copy takes uniform operands; per-thread values would
-     * make the compiler wrap it in a broadcast loop) */
+     * make the compiler wrap it in a broadcast loop).  The copies go to L2 under an evict-first policy ("staging" at the head of
+     * this file); its operands are immediates, so the compiler folds the policy into a constant in uniform registers */
+    uint64_t pol;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
     auto issue = [&](uint32_t k_any) {
         const uint32_t k = __reduce_max_sync(FULL, k_any);
         const uint32_t s = k % NB, dst = win + s * (B * 128), bar = bar0 + s * 8;
         const uint32_t *src = gsrc + (size_t)k * (B * 32);
         if (s == 0) /* slot 0 also refreshes the two mirror rows behind the ring */
             asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\n@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n"
-                         "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%2], [%3], %4, [%0];\n"
-                         "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%5], [%3], 256, [%0];\n}"
-                         ::"r"(bar), "r"(B * 128 + 256u), "r"(dst), "l"(src), "r"(B * 128), "r"(win + NW * 128) : "memory");
+                         "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%2], [%3], %4, [%0], %6;\n"
+                         "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%5], [%3], 256, [%0], %6;\n}"
+                         ::"r"(bar), "r"(B * 128 + 256u), "r"(dst), "l"(src), "r"(B * 128), "r"(win + NW * 128), "l"(pol) : "memory");
         else
             asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\n@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n"
-                         "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%2], [%3], %1, [%0];\n}"
-                         ::"r"(bar), "r"(B * 128), "r"(dst), "l"(src) : "memory");
+                         "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%2], [%3], %1, [%0], %4;\n}"
+                         ::"r"(bar), "r"(B * 128), "r"(dst), "l"(src), "l"(pol) : "memory");
     };
     {
         const uint32_t first = total_b < NB ? total_b : NB;
@@ -347,7 +357,13 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
     uint64_t val = 0;
 
     /* first batch must land before the first value is read */
+#ifdef OG_IL_STATS
+    long long st_w0 = clock64();
+#endif
     if (issued_b && !mbar_wait(bar0, 0)) hung = 1; else ready_b = issued_b ? 1 : 0;
+#ifdef OG_IL_STATS
+    st_wait += clock64() - st_w0;
+#endif
     if (active && !hung) {
         val = fetch64(col, 0); qp = 64; /* first value: 64 raw bits */
         if (rawx) { MASK = ~0ull; kfast = 64; } /* transcoded raw page: a 64-bit XOR delta per row, no control bits */
@@ -459,8 +475,14 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
         const uint32_t qmax = __reduce_max_sync(FULL, done ? 0u : qp);
         uint32_t need_max = ((qmax + OG_IL_LOOKBITS) >> 5) + 1; if (need_max > rows_w) need_max = rows_w;
         uint32_t want_b = (need_max + B - 1) / B; if (want_b > issued_b) want_b = issued_b;
+#ifdef OG_IL_STATS
+        st_w0 = clock64();
+#endif
 #pragma unroll 1
         while (ready_b < want_b) { if (!mbar_wait(bar0 + (ready_b % NB) * 8, (ready_b / NB) & 1)) { hung = 1; break; } ready_b++; }
+#ifdef OG_IL_STATS
+        st_wait += clock64() - st_w0;
+#endif
         if (hung) break;
         uint32_t need = ((qp + OG_IL_LOOKBITS) >> 5) + 1; if (need > rows_w) need = rows_w;
         bool go = done || need <= ready_b * B; /* a lane that could touch rows not resident yet sits the round out */
@@ -534,6 +556,12 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
         ch.edge_bucket[e] = head_b;
         ch.edge_bucket[e + 1] = (head_b == OG_NO_BUCKET || cur_b == head_b) ? OG_NO_BUCKET : cur_b;
     }
+#ifdef OG_IL_STATS
+    if (lane == 0) {
+        atomicAdd((unsigned long long *)(ch.err + 8), (unsigned long long)st_wait);
+        atomicAdd((unsigned long long *)(ch.err + 10), (unsigned long long)(clock64() - st_clk0));
+    }
+#endif
 }
 
 } // namespace ogpu
