@@ -71,9 +71,6 @@ __device__ __forceinline__ void store_cell(const ChunkP &ch, int call, uint32_t 
 /* ------------------------------------------------------------------------------------------------------------
  * shard open: row counts, codec support and framing validation (one thread per segment)
  * ------------------------------------------------------------------------------------------------------------ */
-/* last time of a page and whether its times ascend (segments hold time-ordered rows, lib/record/record.go sort order) */
-struct LastTime { int64_t last; int unsorted = 0; __device__ __forceinline__ void operator()(uint32_t i, int64_t t) { if (i && t < last) unsorted = 1; last = t; } };
-
 __global__ void k_validate(DirP d, const int32_t *col_types, uint32_t *seg_rows, unsigned long long *totals /*[0]=rows [1]=page bytes [2]=time pages that are not const-delta / one-row*/,
                            uint32_t *max_rows, int *err) {
     uint32_t seg = blockIdx.x * blockDim.x + threadIdx.x;
@@ -83,10 +80,14 @@ __global__ void k_validate(DirP d, const int32_t *col_types, uint32_t *seg_rows,
     int rc = parse_time_page(d.data + d.page_off[ti], d.page_len[ti], t);
     if (rc == D_OK && t.rows == 0) rc = D_CORRUPT;
     if (rc == D_OK) { /* the directory's time range must cover the page's times: bucket indices are derived from it and never re-checked */
-        LastTime lt; lt.last = t.t0;
-        if (t.kind == 0) lt.last = (int64_t)((uint64_t)t.t0 + (uint64_t)(t.rows - 1) * t.delta); /* const-delta: closed form */
-        else rc = decode_time_values(t, lt);
-        if (rc == D_OK && (t.t0 < d.seg_tmin[seg] || lt.last > d.seg_tmax[seg] || lt.last < t.t0 || lt.unsorted)) rc = D_CORRUPT;
+        int64_t last = t.t0; bool unsorted = false; /* times must ascend (segments hold time-ordered rows, lib/record/record.go sort order) */
+        if (t.kind == 0) last = (int64_t)((uint64_t)t.t0 + (uint64_t)(t.rows - 1) * t.delta); /* const-delta: closed form */
+        else {
+            TimeIter it; it.init(t);
+            for (uint32_t i = 0; i < t.rows; i++) { const int64_t x = it.next(); unsorted |= x < last; last = x; }
+            it.finish(); rc = it.err;
+        }
+        if (rc == D_OK && (t.t0 < d.seg_tmin[seg] || last > d.seg_tmax[seg] || last < t.t0 || unsorted)) rc = D_CORRUPT;
     }
     if (rc != D_OK) { report_err(err, rc, seg); seg_rows[seg] = 0; return; }
     seg_rows[seg] = t.rows;
@@ -99,6 +100,8 @@ __global__ void k_validate(DirP d, const int32_t *col_types, uint32_t *seg_rows,
         PageHdr h;
         rc = parse_field_header(d.data + d.page_off[pi], len, col_types[c], t.rows, h);
         if (rc == D_OK && h.rows != t.rows) rc = D_CORRUPT;
+        /* the decoders take one value per valid row: the bitmap must mark exactly the header's value count */
+        if (rc == D_OK && h.bitmap && hdr_valid_rows(h) != h.rows - h.nil_count) rc = D_CORRUPT;
         if (rc == D_OK && !h.one_row && h.nil_count < h.rows) {
             if (h.block_len < 1) rc = D_CORRUPT;
             else {
@@ -139,15 +142,6 @@ struct TileP {
     uint8_t *keep;
 };
 
-struct ExpandEmit {
-    uint64_t *out; uint8_t *okb; const PageHdr *h; uint32_t row; size_t stride;
-    __device__ __forceinline__ void operator()(uint32_t, uint64_t bits) {
-        while (row < h->rows && !hdr_row_valid(*h, row)) { out[row * stride] = 0; okb[row * stride] = 0; row++; }
-        if (row < h->rows) { out[row * stride] = bits; okb[row * stride] = 1; row++; }
-    }
-};
-struct TimeStore { int64_t *out; size_t stride; __device__ __forceinline__ void operator()(uint32_t i, int64_t t) { out[i * stride] = t; } };
-
 __global__ void k_decode_tile(DirP d, QueryP q, TileP tp, int *err) {
     uint32_t seg = tp.tile_begin + blockIdx.x * blockDim.x + threadIdx.x;
     if (seg >= tp.tile_end) return;
@@ -158,23 +152,21 @@ __global__ void k_decode_tile(DirP d, QueryP q, TileP tp, int *err) {
         size_t ti = (size_t)d.n_columns * d.n_segments + seg;
         TimeDesc t;
         int rc = parse_time_page(d.data + d.page_off[ti], d.page_len[ti], t);
-        if (rc == D_OK) { TimeStore ts{tp.times + base, S}; rc = decode_time_values(t, ts); }
+        if (rc == D_OK) {
+            TimeIter it; it.init(t);
+            for (uint32_t i = 0; i < t.rows; i++) tp.times[base + i * S] = it.next();
+            it.finish(); rc = it.err;
+        }
         if (rc != D_OK) report_err(err, rc, seg);
         return;
     }
-    int col = q.col_index[slot], type = q.col_type[slot];
-    size_t pi = (size_t)col * d.n_segments + seg;
+    size_t pi = (size_t)q.col_index[slot] * d.n_segments + seg;
     uint64_t *out = tp.vals[slot] + base; uint8_t *okb = tp.okb[slot] + base;
-    uint32_t len = d.page_len[pi];
-    if (len == 0) { for (uint32_t i = 0; i < rows; i++) { out[i * S] = 0; okb[i * S] = 0; } return; }
-    PageHdr h;
-    int rc = parse_field_header(d.data + d.page_off[pi], len, type, rows, h);
-    if (rc == D_OK) {
-        ExpandEmit em{out, okb, &h, 0, S};
-        rc = decode_block(type, h, em);
-        for (uint32_t i = em.row; i < rows; i++) { out[i * S] = 0; okb[i * S] = 0; }
-    }
-    if (rc != D_OK) report_err(err, rc, seg);
+    ColIter it;
+    it.init(d.data + d.page_off[pi], d.page_len[pi], q.col_type[slot], rows);
+    for (uint32_t i = 0; i < rows; i++) { uint64_t v = 0; okb[i * S] = it.next(v); out[i * S] = v; } /* null rows: 0, validity 0 */
+    it.finish();
+    if (it.err != D_OK) report_err(err, it.err, seg);
 }
 
 /* step 2: row mask = inside [tmin,tmax] AND WHERE RPN (one thread per row; SURVEY App.B.12 semantics) */

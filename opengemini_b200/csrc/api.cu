@@ -9,7 +9,6 @@
 #include <numeric>
 
 #include "agg_kernels.cuh"
-#include "fused.cuh"
 #include "il_build.cuh"
 #include "fused_multi.cuh"
 #include "fused_cols.cuh"
@@ -1043,8 +1042,6 @@ OG_API int og_query_next(og_query *q, og_record_view *out) {
 /* =============================================== materialise path =============================================== */
 } /* extern "C" */
 namespace {
-struct DenseEmit { uint8_t *out; int wide; __device__ __forceinline__ void operator()(uint32_t i, uint64_t bits) { if (wide) ((uint64_t *)out)[i] = bits; else out[i] = (uint8_t)bits; } };
-
 /* decode [seg_begin, seg_end) of one column into dense non-null values (ColVal.Val layout, reader.go:504-579) */
 __global__ void k_decode_column(DirP d, uint32_t column, int type, uint32_t seg_begin, uint32_t seg_end, uint8_t *out, uint64_t stride,
                                 uint32_t *rows_out, uint8_t *bitmap_out, uint32_t bitmap_stride, int *err) {
@@ -1056,7 +1053,11 @@ __global__ void k_decode_column(DirP d, uint32_t column, int type, uint32_t seg_
     if (column == d.n_columns) { /* time column */
         TimeDesc t;
         int rc = parse_time_page(d.data + d.page_off[pi], d.page_len[pi], t);
-        if (rc == D_OK) { TimeStore ts{(int64_t *)o, 1}; rc = decode_time_values(t, ts); }
+        if (rc == D_OK) {
+            TimeIter it; it.init(t);
+            for (uint32_t i = 0; i < t.rows; i++) ((int64_t *)o)[i] = it.next();
+            it.finish(); rc = it.err;
+        }
         if (rc != D_OK) report_err(err, rc, seg);
         if (rows_out) rows_out[seg - seg_begin] = rows;
         return;
@@ -1068,11 +1069,18 @@ __global__ void k_decode_column(DirP d, uint32_t column, int type, uint32_t seg_
         if (bm) for (uint32_t i = 0; i < (rows + 7) / 8; i++) bm[i] = 0;
         return;
     }
-    PageHdr h;
-    int rc = parse_field_header(d.data + d.page_off[pi], len, type, rows, h);
+    ColIter it;
+    it.init(d.data + d.page_off[pi], len, type, rows);
+    int rc = it.err;
+    if (rc == D_OK && type == OG_TYPE_STRING) rc = D_UNSUPPORTED; /* string values are never decoded on the device */
     if (rc == D_OK) {
-        DenseEmit em{o, type != OG_TYPE_BOOL};
-        rc = decode_block(type, h, em);
+        const PageHdr &h = it.h;
+        for (uint32_t r = 0, j = 0; r < rows; r++) {
+            uint64_t v;
+            if (!it.next(v)) continue;
+            if (type == OG_TYPE_BOOL) o[j++] = (uint8_t)v; else ((uint64_t *)o)[j++] = v;
+        }
+        it.finish(); rc = it.err;
         if (rows_out) rows_out[seg - seg_begin] = h.rows - h.nil_count;
         if (bm) { /* AppendBitmap re-packed at offset 0 (lib/record/column.go:79-112) */
             for (uint32_t i = 0; i < (rows + 7) / 8; i++) {

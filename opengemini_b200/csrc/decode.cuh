@@ -1,20 +1,27 @@
 /*
- * decode.cuh — device-side page parsing and column block decoders (sm_90a).
+ * decode.cuh — device-side page parsing and the generic page decoders (sm_90a).
  *
- * One thread owns one page and walks it sequentially, handing each decoded value to an `emit(i, bits)` functor,
- * so the same decoders serve the materialise kernels (emit = store) and the fused aggregate kernels
- * (emit = accumulate).  Formats follow SURVEY.md App.A; reference functions replaced:
+ * One thread owns one segment and pulls its rows in order: TimeIter::next() yields the time of the next row, ColIter::next()
+ * the (valid, value) of the next row of one field column, straight from the page bytes.  Every generic consumer — shard
+ * validation, the materialise kernels, the decode step of the tile path and the pull-iterator aggregate kernel — uses these
+ * two iterators, so they all agree on what a corrupt page is.  A consumer that walks a page to its last row calls finish(),
+ * which checks that the words / runs hold exactly the page's value count.  The one exception is k_fused_cols (fused_cols.cuh):
+ * it decodes Gorilla, Simple8b and bool pages in loops of its own, pulls the other codecs through ColIter::value(), and does
+ * not run the end-of-page checks.  Shard open (k_validate) guarantees that a page's validity bits mark exactly
+ * rows - nil_count rows valid, so no iterator takes more values from a block than its header counts.  Formats follow
+ * SURVEY.md App.A; reference functions replaced:
  *   parse_field_header   engine/immutable/column_builder.go:446-486 DecodeColumnHeader, reader.go:700 DecodeColumnOfOneValue
- *   decode_float_block   lib/compress/float.go:139 AdaptiveDecoding; tsm1/batch_float.go:278 FloatArrayDecodeAll;
+ *   ColIter (float)      lib/compress/float.go:139 AdaptiveDecoding; tsm1/batch_float.go:278 FloatArrayDecodeAll;
  *                        lib/compress/compress.go:51,95 SameValueDecoding / RLE.Decoding
- *   decode_int_block     lib/encoding/int.go:370 Integer.Decoding (:214 const-delta, :256 simple8b, :316 raw)
- *   decode_time_*        lib/encoding/timestamp.go:310 Time.Decoding (:190, :227, :299)
- *   decode_bool_block    lib/encoding/bool.go:63 Boolean.Decoding
+ *   ColIter (int)        lib/encoding/int.go:370 Integer.Decoding (:214 const-delta, :256 simple8b, :316 raw)
+ *   ColIter (bool)       lib/encoding/bool.go:63 Boolean.Decoding
+ *   parse_time_page, TimeIter   lib/encoding/timestamp.go:310 Time.Decoding (:190, :227, :299)
  * Unsupported on the device (reported at shard open, never silently skipped): float snappy(2)/mlf(6),
- * int zstd(3), time snappy(3), strings.
+ * int zstd(3), time snappy(3), string values.
  */
 #pragma once
 #include <cstdint>
+#include "../../include/ogpu.h"
 
 namespace ogpu {
 
@@ -111,21 +118,6 @@ __device__ inline int snappy_decode_dev(const uint8_t *in, uint32_t len, uint8_t
     return D_OK;
 }
 
-/* ---------------- MSB-first bit reader over an unaligned byte stream ---------------- */
-struct BitReader {
-    const uint8_t *p; uint64_t pos; uint64_t nbits;
-    __device__ __forceinline__ bool has(unsigned k) const { return pos + k <= nbits; }
-    /* next k (1..64) bits, MSB first; caller guarantees has(k) */
-    __device__ __forceinline__ uint64_t read(unsigned k) {
-        const uint8_t *b = p + (pos >> 3);
-        unsigned sh = (unsigned)(pos & 7);
-        uint64_t w = ld_be64(b) << sh;
-        if (sh && sh + k > 64) w |= (uint64_t)__ldg(b + 8) >> (8 - sh);
-        pos += k;
-        return w >> (64 - k);
-    }
-};
-
 /* ---------------- column segment header ---------------- */
 struct PageHdr {
     uint32_t rows;          /* Len */
@@ -175,6 +167,16 @@ __device__ __forceinline__ bool hdr_row_valid(const PageHdr &h, uint32_t i) {
     if (!h.bitmap) return h.nil_count == 0;
     uint32_t b = h.bm_off + i;
     return (__ldg(h.bitmap + (b >> 3)) >> (b & 7)) & 1;
+}
+/* number of rows the validity bits mark valid (a page with a bitmap) */
+__device__ __forceinline__ uint32_t hdr_valid_rows(const PageHdr &h) {
+    uint32_t n = 0;
+    for (uint32_t i = 0; i < h.rows;) {
+        const uint32_t b = h.bm_off + i, k = min(8u - (b & 7), h.rows - i);
+        n += __popc((__ldg(h.bitmap + (b >> 3)) >> (b & 7)) & ((1u << k) - 1));
+        i += k;
+    }
+    return n;
 }
 
 /* ---------------- time pages ---------------- */
@@ -235,181 +237,189 @@ __device__ __forceinline__ void s8b_sel(unsigned sel, unsigned &n, unsigned &bit
     n = N[sel]; bits = B[sel];
 }
 
-/* sequential time decode; emit(i, t).  Returns D_OK or D_CORRUPT. */
-template <class Emit>
-__device__ __forceinline__ int decode_time_values(const TimeDesc &t, Emit &&emit) {
-    if (t.kind == 0 || t.kind == 3) {
-        uint64_t cur = (uint64_t)t.t0;
-        for (uint32_t i = 0; i < t.rows; i++) { emit(i, (int64_t)cur); cur += t.delta; }
-        return D_OK;
-    }
-    if (t.kind == 2) {
-        for (uint32_t i = 0; i < t.rows; i++) emit(i, zigzag_dec(ld_be64(t.words + 8ull * i)));
-        return D_OK;
-    }
-    uint64_t cur = (uint64_t)t.t0; uint32_t idx = 0;
-    emit(idx++, (int64_t)cur);
-    for (uint32_t w = 0; w < t.n_words; w++) {
-        uint64_t v = ld_be64(t.words + 8ull * w);
-        unsigned n, bits; s8b_sel((unsigned)(v >> 60), n, bits);
-        uint64_t mask = bits == 0 ? 0 : ((1ull << bits) - 1);
-        for (unsigned k = 0; k < n; k++) {
-            if (idx >= t.rows) return D_CORRUPT;
-            uint64_t d = bits == 0 ? 1ull : ((v >> (k * bits)) & mask);
-            cur += d * t.delta;
-            emit(idx++, (int64_t)cur);
+/* time of the next row of a time page; rows past t.rows must not be pulled */
+struct TimeIter {
+    TimeDesc d; uint64_t cur; uint32_t idx; uint32_t w; unsigned k, n, bits; uint64_t word;
+    int err;
+    __device__ __forceinline__ void init(const TimeDesc &t) { d = t; cur = (uint64_t)t.t0; idx = 0; w = 0; k = 0; n = 0; bits = 0; word = 0; err = D_OK; }
+    __device__ __forceinline__ int64_t next() { /* time of row idx, then advance */
+        int64_t t;
+        if (d.kind == 0 || d.kind == 3) { t = (int64_t)cur; cur += d.delta; }
+        else if (d.kind == 2) { t = zigzag_dec(ld_be64(d.words + 8ull * idx)); }
+        else {
+            if (idx != 0) {
+                while (k == n) { /* next simple8b word */
+                    if (w >= d.n_words) { err = D_CORRUPT; idx++; return (int64_t)cur; } /* fewer deltas than rows */
+                    word = ld_be64(d.words + 8ull * w); w++;
+                    s8b_sel((unsigned)(word >> 60), n, bits); k = 0;
+                }
+                uint64_t dv = bits == 0 ? 1ull : ((word >> (k * bits)) & ((1ull << bits) - 1));
+                k++;
+                cur += dv * d.delta;
+            }
+            t = (int64_t)cur;
         }
+        idx++;
+        return t;
     }
-    return idx == t.rows ? D_OK : D_CORRUPT;
-}
+    /* after the last row: a Simple8b page holds exactly rows - 1 deltas (timestamp.go:267) */
+    __device__ __forceinline__ void finish() {
+        if (d.kind == 1 && (w != d.n_words || k != n)) err = D_CORRUPT;
+    }
+};
 
-/* ---------------- float blocks ---------------- */
+/* ---------------- field pages ---------------- */
 #define OG_UVNAN 0x7FF8000000000001ull
 
-/* n = number of non-null values expected (rows - nilCount).  emit(i, bits). */
-template <class Emit>
-__device__ __forceinline__ int decode_float_block(const uint8_t *in, uint32_t len, uint32_t n, Emit &&emit) {
-    if (n == 0) return D_OK;
-    if (len < 1) return D_CORRUPT;
-    int algo = __ldg(in) >> 4;
-    const uint8_t *b = in + 1; uint32_t bl = len - 1;
-    switch (algo) {
-    case 0: { /* floatCompressedNull: raw LE */
-        if (bl < 8ull * n) return D_CORRUPT;
-        for (uint32_t i = 0; i < n; i++) emit(i, ld_le64(b + 8ull * i));
-        return D_OK;
+/* next (valid, value) of one field column of one segment; value = raw 64-bit cell (double bits / int64 / bool 0,1) */
+struct ColIter {
+    enum { K_ABSENT = 0, K_NULLMAP /* string column: validity only, values are never decoded */, K_ONE, K_F_RAW, K_F_GORILLA, K_F_SAME, K_F_RLE, K_I_CONST, K_I_S8B, K_I_RAW, K_B_BITS };
+    PageHdr h;
+    int kind, type;
+    uint32_t row;      /* next row */
+    uint32_t idx;      /* next non-null value */
+    const uint8_t *p;  /* payload cursor (codec specific) */
+    uint64_t cur;      /* current value / run value / accumulator */
+    uint64_t aux;      /* gorilla: bit position; s8b: current word; const: delta */
+    uint32_t a, b, c;  /* gorilla: trailing, meaningful, bits in stream; s8b: k, n, bits; rle: run left, -, bytes left */
+    uint32_t words_left;
+    int err;
+
+    __device__ __forceinline__ void init(const uint8_t *page, uint32_t len, int col_type, uint32_t seg_rows) {
+        type = col_type; row = 0; idx = 0; err = D_OK; cur = 0; aux = 0; a = b = c = 0; words_left = 0; p = nullptr;
+        if (len == 0) { kind = K_ABSENT; h.rows = seg_rows; h.nil_count = seg_rows; h.bitmap = nullptr; h.bm_off = 0; h.block = nullptr; h.block_len = 0; h.one_row = 0; return; }
+        int rc = parse_field_header(page, len, col_type, seg_rows, h);
+        if (rc != D_OK) { err = rc; kind = K_ABSENT; return; }
+        const uint32_t n = h.rows - h.nil_count;
+        if (n == 0) { kind = K_ABSENT; return; }
+        if (col_type == OG_TYPE_STRING) { kind = K_NULLMAP; return; } /* lib/encoding/string.go:286-302 is not needed for count(): ValidCount reads the bitmap */
+        if (h.one_row) { kind = K_ONE; cur = col_type == OG_TYPE_BOOL ? (uint64_t)__ldg(h.block) : (h.block_len >= 8 ? ld_le64(h.block) : 0); if (col_type != OG_TYPE_BOOL && h.block_len < 8) err = D_CORRUPT; return; }
+        if (h.block_len < 1) { err = D_CORRUPT; kind = K_ABSENT; return; }
+        const uint8_t *in = h.block; const uint32_t bl = h.block_len - 1;
+        const int tag = __ldg(in) >> 4;
+        p = in + 1;
+        if (col_type == OG_TYPE_FLOAT) {
+            switch (tag) {
+            case 0: kind = K_F_RAW; if (bl < 8ull * n) err = D_CORRUPT; break;
+            case 3: kind = K_F_GORILLA;
+                if (bl < 9) { err = D_CORRUPT; break; }
+                cur = ld_be64(p + 1); p += 9; aux = 0; a = 0; b = 64; c = (bl - 9) * 8;
+                if (cur == OG_UVNAN) err = D_CORRUPT;
+                break;
+            case 4: kind = K_F_SAME; if (bl < 2 || ld_be16(p) != n) { err = D_CORRUPT; break; } cur = 0; if (bl != 2) { if (bl < 10) err = D_CORRUPT; else cur = ld_le64(p + 2); } break;
+            case 5: kind = K_F_RLE; a = 0; c = bl; break;
+            default: err = (tag == 1 || tag == 2 || tag == 6) ? D_UNSUPPORTED : D_CORRUPT; break;
+            }
+        } else if (col_type == OG_TYPE_INT) {
+            if (bl < 4) { err = D_CORRUPT; kind = K_ABSENT; return; }
+            switch (tag) {
+            case 4: kind = K_I_RAW; if (bl - 4 < ld_be32(p) || (bl - 4) / 8 != n) err = D_CORRUPT; p += 4; break;
+            case 1: { kind = K_I_CONST;
+                if (bl < 8) { err = D_CORRUPT; break; }
+                uint64_t d, cnt; int k = ld_uvarint(p + 8, bl - 8, &d);
+                int k2 = k ? ld_uvarint(p + 8 + k, bl - 8 - k, &cnt) : 0;
+                if (k == 0 || k2 == 0 || cnt + 1 != n) { err = D_CORRUPT; break; }
+                cur = (uint64_t)zigzag_dec(ld_be64(p)); aux = (uint64_t)zigzag_dec(d);
+                break; }
+            case 2: { kind = K_I_S8B;
+                if (bl < 16) { err = D_CORRUPT; break; }
+                const uint32_t enc = ld_be32(p), src = ld_be32(p + 4);
+                if (src != n || enc == 0 || bl - 8 < enc * 8ull) { err = D_CORRUPT; break; }
+                cur = (uint64_t)zigzag_dec(ld_be64(p + 8)); p += 16; words_left = enc - 1; a = 0; b = 0; c = 0;
+                break; }
+            default: err = tag == 3 ? D_UNSUPPORTED : D_CORRUPT; break;
+            }
+        } else if (col_type == OG_TYPE_BOOL) {
+            kind = K_B_BITS;
+            if (tag != 1 || bl < 4 || ld_be32(p) != n || (uint64_t)(bl - 4) * 8 < n) err = D_CORRUPT;
+            p += 4;
+        } else err = D_UNSUPPORTED;
+        if (err != D_OK) kind = K_ABSENT;
     }
-    case 3: { /* Gorilla: [0x10][8 B BE first][bit stream] */
-        if (bl < 9) return D_CORRUPT;
-        uint64_t val = ld_be64(b + 1);
-        if (val == OG_UVNAN) return D_CORRUPT; /* empty stream but values expected */
-        emit(0, val);
-        BitReader br{b + 9, 0, (uint64_t)(bl - 9) * 8};
-        unsigned trailing = 0, meaningful = 64;
-        for (uint32_t i = 1; i < n; i++) {
-            if (!br.has(1)) return D_CORRUPT;
-            if (br.read(1)) {
-                if (!br.has(1)) return D_CORRUPT;
-                if (br.read(1)) {
-                    if (!br.has(11)) return D_CORRUPT;
-                    unsigned lm = (unsigned)br.read(11);
-                    unsigned leading = (lm >> 6) & 0x1f;
-                    meaningful = lm & 0x3f;
-                    if (meaningful > 0) { if (leading + meaningful > 64) return D_CORRUPT; trailing = 64 - leading - meaningful; }
-                    else { trailing = 0; meaningful = 64; }
+
+    /* value of the next non-null row (idx-th value of the block) */
+    __device__ __forceinline__ uint64_t value() {
+        const uint32_t i = idx++;
+        switch (kind) {
+        case K_ONE: return cur;
+        case K_F_RAW: return ld_le64(p + 8ull * i);
+        case K_F_SAME: return cur;
+        case K_F_GORILLA: {
+            if (i == 0) return cur;
+            /* one record of tsm1.FloatArrayDecodeAll (batch_float.go:352-508).  '0' (same value) and '10' (window reuse) are
+             * handled without a branch — a '0' is a record with zero meaningful bits — so lanes of a warp that sit on different
+             * record kinds do not serialise; only the rare '11' (new window) branches. */
+            const uint8_t *bp = p + (aux >> 3);
+            const unsigned sh = (unsigned)(aux & 7);
+            const uint64_t w = ld_be64(bp) << sh; /* >= 57 valid bits */
+            unsigned used = (w >> 63) ? 2u : 1u;
+            if ((w >> 62) == 3) {
+                const unsigned lm = (unsigned)(w >> 51) & 0x7ff;
+                const unsigned lead = (lm >> 6) & 0x1f;
+                b = lm & 0x3f;
+                if (b > 0) { if (lead + b > 64) { err = D_CORRUPT; b = 64; a = 0; } else a = 64 - lead - b; }
+                else { a = 0; b = 64; }
+                used = 13;
+            }
+            const unsigned mb = (w >> 63) ? b : 0u; /* meaningful bits of this record */
+            aux += used;
+            const uint8_t *q2 = p + (aux >> 3);
+            const unsigned s2 = (unsigned)(aux & 7);
+            uint64_t v = ld_be64(q2) << s2;
+            if (s2 + mb > 64) v |= (uint64_t)__ldg(q2 + 8) >> (8 - s2);
+            v = mb == 64 ? v : mb == 0 ? 0ull : (v >> (64 - mb));
+            aux += mb;
+            if (aux > c) { err = D_CORRUPT; aux = c; return cur; } /* truncated stream: later rows keep reading at its end, not past it */
+            cur ^= v << a;
+            if (mb && cur == OG_UVNAN) err = D_CORRUPT; /* sentinel before the block's value count */
+            return cur; }
+        case K_F_RLE: {
+            while (a == 0) { /* next run: [u16 BE n (bit15 = zero run)][8 B LE] (compress.go:95-120) */
+                if (c < 2) { err = D_CORRUPT; return 0; }
+                const uint32_t n = ld_be16(p);
+                if (n >> 15) { a = n - (1u << 15); cur = 0; p += 2; c -= 2; } /* a zero run of length 0 pads nothing (:105-110) */
+                else { /* a value run of length 0 has no defined result in paddingBuffer (:171-187) */
+                    if (c < 10 || n == 0) { err = D_CORRUPT; return 0; }
+                    a = n; cur = ld_le64(p + 2); p += 10; c -= 10;
                 }
-                if (!br.has(meaningful)) return D_CORRUPT;
-                val ^= br.read(meaningful) << trailing;
-                if (val == OG_UVNAN) return D_CORRUPT; /* sentinel before n values */
             }
-            emit(i, val);
-        }
-        return D_OK;
-    }
-    case 4: { /* Same: [u16 BE count][8 B LE value, absent when 0] */
-        if (bl < 2) return D_CORRUPT;
-        uint32_t cnt = ld_be16(b);
-        if (cnt != n) return D_CORRUPT;
-        uint64_t v = 0;
-        if (bl != 2) { if (bl < 10) return D_CORRUPT; v = ld_le64(b + 2); }
-        for (uint32_t i = 0; i < n; i++) emit(i, v);
-        return D_OK;
-    }
-    case 5: { /* RLE: repeat [u16 BE n (bit15 = zero run)][8 B LE] */
-        uint32_t idx = 0;
-        while (bl >= 2) {
-            uint32_t c = ld_be16(b);
-            uint64_t v = 0;
-            if (c >> 15) { c -= 1u << 15; b += 2; bl -= 2; }
-            else { if (bl < 10) return D_CORRUPT; v = ld_le64(b + 2); b += 10; bl -= 10; }
-            if (idx + c > n) return D_CORRUPT;
-            for (uint32_t k = 0; k < c; k++) emit(idx++, v);
-        }
-        return idx == n ? D_OK : D_CORRUPT;
-    }
-    case 1: case 2: case 6: return D_UNSUPPORTED; /* legacy gorilla, snappy, mlf */
-    default: return D_CORRUPT;
-    }
-}
-
-/* ---------------- int blocks ---------------- */
-template <class Emit>
-__device__ __forceinline__ int decode_int_block(const uint8_t *in, uint32_t len, uint32_t n, Emit &&emit) {
-    if (n == 0) return D_OK;
-    if (len < 5) return D_CORRUPT;
-    int ty = __ldg(in) >> 4;
-    const uint8_t *b = in + 1; uint32_t bl = len - 1;
-    switch (ty) {
-    case 4: { /* raw: [u32 byteLen][n x u64 BE zigzag] */
-        uint32_t byte_len = ld_be32(b);
-        if (bl - 4 < byte_len || (bl - 4) / 8 != n) return D_CORRUPT;
-        for (uint32_t i = 0; i < n; i++) emit(i, (uint64_t)zigzag_dec(ld_be64(b + 4 + 8ull * i)));
-        return D_OK;
-    }
-    case 1: { /* const delta */
-        if (bl < 8) return D_CORRUPT;
-        uint64_t first = ld_be64(b), d, c;
-        int k = ld_uvarint(b + 8, bl - 8, &d);
-        if (k == 0) return D_CORRUPT;
-        int k2 = ld_uvarint(b + 8 + k, bl - 8 - k, &c);
-        if (k2 == 0 || c + 1 != n) return D_CORRUPT;
-        uint64_t cur = (uint64_t)zigzag_dec(first), dv = (uint64_t)zigzag_dec(d);
-        for (uint32_t i = 0; i < n; i++) { emit(i, cur); cur += dv; }
-        return D_OK;
-    }
-    case 2: { /* simple8b: [u32 encCnt][u32 srcCnt][u64 BE zz(v0)][words] */
-        if (bl < 16) return D_CORRUPT;
-        uint32_t enc = ld_be32(b), src = ld_be32(b + 4);
-        if (src != n || enc == 0 || bl - 8 < enc * 8ull) return D_CORRUPT;
-        uint64_t cur = (uint64_t)zigzag_dec(ld_be64(b + 8));
-        uint32_t idx = 0;
-        emit(idx++, cur);
-        const uint8_t *w = b + 16;
-        for (uint32_t wi = 0; wi + 1 < enc; wi++) {
-            uint64_t v = ld_be64(w + 8ull * wi);
-            unsigned cnt, bits; s8b_sel((unsigned)(v >> 60), cnt, bits);
-            uint64_t mask = bits == 0 ? 0 : ((1ull << bits) - 1);
-            for (unsigned k = 0; k < cnt; k++) {
-                if (idx >= n) return D_CORRUPT;
-                uint64_t z = bits == 0 ? 1ull : ((v >> (k * bits)) & mask);
-                cur += (uint64_t)zigzag_dec(z);
-                emit(idx++, cur);
+            a--;
+            return cur; }
+        case K_I_RAW: return (uint64_t)zigzag_dec(ld_be64(p + 8ull * i));
+        case K_I_CONST: { const uint64_t v = cur; cur += aux; return v; }
+        case K_I_S8B: {
+            if (i == 0) return cur;
+            while (a == b) { /* next simple8b word (simple8b/encoding.go:193-210) */
+                if (words_left == 0) { err = D_CORRUPT; return cur; }
+                aux = ld_be64(p); p += 8; words_left--;
+                unsigned nn, bits; s8b_sel((unsigned)(aux >> 60), nn, bits);
+                b = nn; c = bits; a = 0;
             }
+            const uint64_t z = c == 0 ? 1ull : ((aux >> (a * c)) & ((1ull << c) - 1));
+            a++;
+            cur += (uint64_t)zigzag_dec(z);
+            return cur; }
+        case K_B_BITS: return (uint64_t)((__ldg(p + (i >> 3)) >> (7 - (i & 7))) & 1);
+        default: return 0;
         }
-        return idx == n ? D_OK : D_CORRUPT;
     }
-    case 3: return D_UNSUPPORTED; /* zstd */
-    default: return D_CORRUPT;
+    __device__ __forceinline__ bool next(uint64_t &v) {
+        const uint32_t r = row++;
+        if (kind == K_ABSENT) return false;
+        if (!hdr_row_valid(h, r)) return false;
+        v = value();
+        return true;
     }
-}
-
-/* ---------------- bool blocks ---------------- */
-template <class Emit>
-__device__ __forceinline__ int decode_bool_block(const uint8_t *in, uint32_t len, uint32_t n, Emit &&emit) {
-    if (n == 0) return D_OK;
-    if (len < 5) return D_CORRUPT;
-    if ((__ldg(in) >> 4) != 1) return D_CORRUPT;
-    uint32_t cnt = ld_be32(in + 1);
-    if (cnt != n || (uint64_t)(len - 5) * 8 < n) return D_CORRUPT;
-    const uint8_t *b = in + 5;
-    for (uint32_t i = 0; i < n; i++) emit(i, (uint64_t)((__ldg(b + (i >> 3)) >> (7 - (i & 7))) & 1));
-    return D_OK;
-}
-
-/* typed dispatch: decodes the n non-null values of a page block */
-template <class Emit>
-__device__ __forceinline__ int decode_block(int type, const PageHdr &h, Emit &&emit) {
-    uint32_t n = h.rows - h.nil_count;
-    if (h.one_row) {
-        if (n == 0) return D_OK;
-        if (type == 5) { emit(0u, (uint64_t)__ldg(h.block)); return D_OK; }
-        if (h.block_len < 8) return D_CORRUPT;
-        emit(0u, ld_le64(h.block)); return D_OK;
+    /* after the last row: the words / runs must hold exactly the block's value count */
+    __device__ __forceinline__ void finish() {
+        const uint32_t n = h.rows - h.nil_count;
+        if (kind == K_I_S8B) { /* every slot of every word taken, and as many values as srcCount (int.go:296) */
+            if (idx != n || a != b || words_left != 0) err = D_CORRUPT;
+        } else if (kind == K_F_RLE) { /* runs add up to n; only zero-length zero runs may follow, and < 2 bytes (compress.go:99-101) */
+            if (idx != n || a != 0) err = D_CORRUPT;
+            for (; c >= 2 && err == D_OK; p += 2, c -= 2) if (ld_be16(p) != 0x8000u) err = D_CORRUPT;
+        }
     }
-    if (type == 3) return decode_float_block(h.block, h.block_len, n, emit);
-    if (type == 1) return decode_int_block(h.block, h.block_len, n, emit);
-    if (type == 5) return decode_bool_block(h.block, h.block_len, n, emit);
-    return D_UNSUPPORTED;
-}
+};
 
 } // namespace ogpu

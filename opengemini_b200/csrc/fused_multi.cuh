@@ -1,167 +1,28 @@
 /*
- * fused_multi.cuh — K5 for queries that touch several field columns and/or carry a WHERE on fields (configs[2]: int64
- * Simple8b + float64 Gorilla + bool columns, count/sum with a filter): fused decode + filter + time-bucket + reduce, one
- * thread per segment, NOTHING materialised.
+ * fused_multi.cuh — K5, the general fused kernels: decode + filter + time-bucket + reduce, one thread per segment, NOTHING
+ * materialised.  k_fused_multi serves the queries that touch several field columns and/or carry a WHERE on fields and that
+ * k_fused_cols does not take (og_stats.path 4); k_fused_segment, its one-column form without a filter, serves single-column
+ * queries over any codec, nulls or time codec (path 1, and the segments k_fused_il leaves over).
  *
- * The generic path writes every decoded column of a tile of segments to HBM (17 B per row and column, written and read
- * back) before it filters and reduces; here each column of the segment is a PULL iterator — ColIter::next() yields the
- * (valid, value) of the next row straight from the page bytes — so a row's columns meet in registers: WHERE is evaluated on
- * them (lib/binaryfilterfunc/functions.go:632 semantics: NULL never matches, ordered tests pass NaN), the surviving row is
- * accumulated into the open window's partials, and only window partials leave the thread (edges / per-series cells, exactly
- * what k_fused_segment writes, so k_fix_edges and the merges are shared).  Pages of these columns are small (0.1-2 KB), a
- * thread walks its pages front to back, and consecutive 8-byte reads of one thread hit the sector/line its previous read
- * brought into L1: DRAM traffic stays at the page bytes.
+ * The tile path writes every decoded column of a tile of segments to HBM (17 B per row and column, written and read back)
+ * before it filters and reduces; here each column of the segment is a PULL iterator (ColIter, decode.cuh) and time comes from
+ * a TimeIter, so a row's columns meet in registers: WHERE is evaluated on them (lib/binaryfilterfunc/functions.go:632
+ * semantics: NULL never matches, ordered tests pass NaN), the surviving row is accumulated into the open window's partials,
+ * and only window partials leave the thread (edges / per-series cells, the layout k_window_reduce and k_fused_cols write, so
+ * k_fix_edges and the merges are shared).  Pages are read front to back, and consecutive 8-byte reads of one thread hit the
+ * sector/line its previous read brought into L1: DRAM traffic stays at the page bytes.
  *
  * Replaces (for <= OG_MULTI_MAXC columns): readSegmentRecord (tssp_file.go:369) + decodeColumnData (reader.go:674) for every
- * codec the single-column kernels know + FilterByTime (reader.go:754) + FilterByField (reader.go:895-974, functions.go:632)
+ * codec the device knows + FilterByTime (reader.go:754) + FilterByField (reader.go:895-974, functions.go:632)
  * + aggregateCursor (aggregate_cursor.go:306-356) + the per-window reducers (series_agg_func.gen.go:24-274).
  */
 #pragma once
-#include "fused.cuh"
+#include "agg_kernels.cuh"
+#include <type_traits>
 
 namespace ogpu {
 
 #define OG_MULTI_MAXC 4
-
-/* next (valid, value) of one field column of one segment; value = raw 64-bit cell (double bits / int64 / bool 0,1) */
-struct ColIter {
-    enum { K_ABSENT = 0, K_NULLMAP /* string column: validity only, values are never decoded */, K_ONE, K_F_RAW, K_F_GORILLA, K_F_SAME, K_F_RLE, K_I_CONST, K_I_S8B, K_I_RAW, K_B_BITS };
-    PageHdr h;
-    int kind, type;
-    uint32_t row;      /* next row */
-    uint32_t idx;      /* next non-null value */
-    const uint8_t *p;  /* payload cursor (codec specific) */
-    uint64_t cur;      /* current value / run value / accumulator */
-    uint64_t aux;      /* gorilla: bit position; s8b: current word; const: delta */
-    uint32_t a, b, c;  /* gorilla: trailing, meaningful, bits in stream; s8b: k, n, bits (+ words left in idx2); rle: run left */
-    uint32_t words_left;
-    int err;
-
-    __device__ __forceinline__ void init(const uint8_t *page, uint32_t len, int col_type, uint32_t seg_rows) {
-        type = col_type; row = 0; idx = 0; err = D_OK; cur = 0; aux = 0; a = b = c = 0; words_left = 0; p = nullptr;
-        if (len == 0) { kind = K_ABSENT; h.rows = seg_rows; h.nil_count = seg_rows; h.bitmap = nullptr; h.bm_off = 0; h.block = nullptr; h.block_len = 0; h.one_row = 0; return; }
-        int rc = parse_field_header(page, len, col_type, seg_rows, h);
-        if (rc != D_OK) { err = rc; kind = K_ABSENT; return; }
-        const uint32_t n = h.rows - h.nil_count;
-        if (n == 0) { kind = K_ABSENT; return; }
-        if (col_type == OG_TYPE_STRING) { kind = K_NULLMAP; return; } /* lib/encoding/string.go:286-302 is not needed for count(): ValidCount reads the bitmap */
-        if (h.one_row) { kind = K_ONE; cur = col_type == OG_TYPE_BOOL ? (uint64_t)__ldg(h.block) : (h.block_len >= 8 ? ld_le64(h.block) : 0); if (col_type != OG_TYPE_BOOL && h.block_len < 8) err = D_CORRUPT; return; }
-        if (h.block_len < 1) { err = D_CORRUPT; kind = K_ABSENT; return; }
-        const uint8_t *in = h.block; const uint32_t bl = h.block_len - 1;
-        const int tag = __ldg(in) >> 4;
-        p = in + 1;
-        if (col_type == OG_TYPE_FLOAT) {
-            switch (tag) {
-            case 0: kind = K_F_RAW; if (bl < 8ull * n) err = D_CORRUPT; break;
-            case 3: kind = K_F_GORILLA;
-                if (bl < 9) { err = D_CORRUPT; break; }
-                cur = ld_be64(p + 1); p += 9; aux = 0; a = 0; b = 64; c = (bl - 9) * 8;
-                if (cur == OG_UVNAN) err = D_CORRUPT;
-                break;
-            case 4: kind = K_F_SAME; if (bl < 2 || ld_be16(p) != n) { err = D_CORRUPT; break; } cur = 0; if (bl != 2) { if (bl < 10) err = D_CORRUPT; else cur = ld_le64(p + 2); } break;
-            case 5: kind = K_F_RLE; a = 0; c = bl; break;
-            default: err = (tag == 1 || tag == 2 || tag == 6) ? D_UNSUPPORTED : D_CORRUPT; break;
-            }
-        } else if (col_type == OG_TYPE_INT) {
-            if (bl < 4) { err = D_CORRUPT; kind = K_ABSENT; return; }
-            switch (tag) {
-            case 4: kind = K_I_RAW; if (bl - 4 < ld_be32(p) || (bl - 4) / 8 != n) err = D_CORRUPT; p += 4; break;
-            case 1: { kind = K_I_CONST;
-                if (bl < 8) { err = D_CORRUPT; break; }
-                uint64_t d, cnt; int k = ld_uvarint(p + 8, bl - 8, &d);
-                int k2 = k ? ld_uvarint(p + 8 + k, bl - 8 - k, &cnt) : 0;
-                if (k == 0 || k2 == 0 || cnt + 1 != n) { err = D_CORRUPT; break; }
-                cur = (uint64_t)zigzag_dec(ld_be64(p)); aux = (uint64_t)zigzag_dec(d);
-                break; }
-            case 2: { kind = K_I_S8B;
-                if (bl < 16) { err = D_CORRUPT; break; }
-                const uint32_t enc = ld_be32(p), src = ld_be32(p + 4);
-                if (src != n || enc == 0 || bl - 8 < enc * 8ull) { err = D_CORRUPT; break; }
-                cur = (uint64_t)zigzag_dec(ld_be64(p + 8)); p += 16; words_left = enc - 1; a = 0; b = 0; c = 0;
-                break; }
-            default: err = tag == 3 ? D_UNSUPPORTED : D_CORRUPT; break;
-            }
-        } else if (col_type == OG_TYPE_BOOL) {
-            kind = K_B_BITS;
-            if (tag != 1 || bl < 4 || ld_be32(p) != n || (uint64_t)(bl - 4) * 8 < n) err = D_CORRUPT;
-            p += 4;
-        } else err = D_UNSUPPORTED;
-        if (err != D_OK) kind = K_ABSENT;
-    }
-
-    /* value of the next non-null row (idx-th value of the block) */
-    __device__ __forceinline__ uint64_t value() {
-        const uint32_t i = idx++;
-        switch (kind) {
-        case K_ONE: return cur;
-        case K_F_RAW: return ld_le64(p + 8ull * i);
-        case K_F_SAME: return cur;
-        case K_F_GORILLA: {
-            if (i == 0) return cur;
-            /* one record of tsm1.FloatArrayDecodeAll (batch_float.go:352-508).  '0' (same value) and '10' (window reuse) are
-             * handled without a branch — a '0' is a record with zero meaningful bits — so lanes of a warp that sit on different
-             * record kinds do not serialise; only the rare '11' (new window) branches. */
-            const uint8_t *bp = p + (aux >> 3);
-            const unsigned sh = (unsigned)(aux & 7);
-            const uint64_t w = ld_be64(bp) << sh; /* >= 57 valid bits */
-            unsigned used = (w >> 63) ? 2u : 1u;
-            if ((w >> 62) == 3) {
-                const unsigned lm = (unsigned)(w >> 51) & 0x7ff;
-                const unsigned lead = (lm >> 6) & 0x1f;
-                b = lm & 0x3f;
-                if (b > 0) { if (lead + b > 64) { err = D_CORRUPT; b = 64; a = 0; } else a = 64 - lead - b; }
-                else { a = 0; b = 64; }
-                used = 13;
-            }
-            const unsigned mb = (w >> 63) ? b : 0u; /* meaningful bits of this record */
-            aux += used;
-            const uint8_t *q2 = p + (aux >> 3);
-            const unsigned s2 = (unsigned)(aux & 7);
-            uint64_t v = ld_be64(q2) << s2;
-            if (s2 + mb > 64) v |= (uint64_t)__ldg(q2 + 8) >> (8 - s2);
-            v = mb == 64 ? v : mb == 0 ? 0ull : (v >> (64 - mb));
-            aux += mb;
-            if (aux > c) { err = D_CORRUPT; return cur; }
-            cur ^= v << a;
-            if (mb && cur == OG_UVNAN) err = D_CORRUPT; /* sentinel before the block's value count */
-            return cur; }
-        case K_F_RLE: {
-            if (a == 0) { /* next run: [u16 BE n (bit15 = zero run)][8 B LE] */
-                if (c < 2) { err = D_CORRUPT; return 0; }
-                uint32_t n = ld_be16(p);
-                if (n >> 15) { n -= 1u << 15; cur = 0; p += 2; c -= 2; }
-                else { if (c < 10) { err = D_CORRUPT; return 0; } cur = ld_le64(p + 2); p += 10; c -= 10; }
-                if (n == 0) { err = D_CORRUPT; return 0; }
-                a = n;
-            }
-            a--;
-            return cur; }
-        case K_I_RAW: return (uint64_t)zigzag_dec(ld_be64(p + 8ull * i));
-        case K_I_CONST: { const uint64_t v = cur; cur += aux; return v; }
-        case K_I_S8B: {
-            if (i == 0) return cur;
-            while (a == b) { /* next simple8b word (simple8b/encoding.go:193-210) */
-                if (words_left == 0) { err = D_CORRUPT; return cur; }
-                aux = ld_be64(p); p += 8; words_left--;
-                unsigned nn, bits; s8b_sel((unsigned)(aux >> 60), nn, bits);
-                b = nn; c = bits; a = 0;
-            }
-            const uint64_t z = c == 0 ? 1ull : ((aux >> (a * c)) & ((1ull << c) - 1));
-            a++;
-            cur += (uint64_t)zigzag_dec(z);
-            return cur; }
-        case K_B_BITS: return (uint64_t)((__ldg(p + (i >> 3)) >> (7 - (i & 7))) & 1);
-        default: return 0;
-        }
-    }
-    __device__ __forceinline__ bool next(uint64_t &v) {
-        const uint32_t r = row++;
-        if (kind == K_ABSENT) return false;
-        if (!hdr_row_valid(h, r)) return false;
-        v = value();
-        return true;
-    }
-};
 
 /* NCALL = number of calls (partials live in registers); SIMPLE = every call is count or sum (the shape configs[2] names): the
  * per-call switch of acc_row collapses to an add */
@@ -199,7 +60,8 @@ __global__ void __launch_bounds__(128) k_fused_multi(DirP d, QueryP q, ChunkP ch
         }
         if (!head_done) { head_done = true; head_b = cur_b; }
     };
-    for (uint32_t r = 0; r < rows; r++) {
+    uint32_t r = 0;
+    for (; r < rows; r++) {
         const int64_t t = ti.next();
         uint64_t v[NCOL]; bool ok[NCOL];
 #pragma unroll
@@ -253,7 +115,98 @@ __global__ void __launch_bounds__(128) k_fused_multi(DirP d, QueryP q, ChunkP ch
             }
         }
     }
+    if (r == rows) { /* the pages were walked to their last row (a scan that stops at tmax leaves the rest unread) */
+        ti.finish();
+#pragma unroll
+        for (int k = 0; k < NCOL; k++) col[k].finish();
+    }
+    if (ti.err != D_OK) report_err(ch.err, ti.err, seg);
     for (int k = 0; k < NCOL; k++) if (col[k].err != D_OK) report_err(ch.err, col[k].err, seg);
+    const uint32_t last_b = cur_b;
+    const bool single = !head_done;
+    flush(true);
+    ch.edge_bucket[e] = head_b;
+    ch.edge_bucket[e + 1] = (single || head_b == OG_NO_BUCKET) ? OG_NO_BUCKET : last_b;
+}
+
+/* One column, no WHERE (og_stats.path 1, and the segments k_fused_il leaves over): the row loop of k_fused_multi without the
+ * filter, run once per codec kind so that ColIter's codec switch folds away.  Sum, count, max over the int64 column of configs[2]
+ * (H100 80GB HBM3, 400 W): this kernel 35.4 ms, k_fused_multi<1, 3, false> 48 ms, the push-decoder kernel it replaced 40.4 ms.  `list` (sorted segment
+ * ids, `n` of them) selects the segments of the chunk that k_fused_il did not take, compacted so that warps stay full;
+ * list == nullptr: every segment of the chunk. */
+template <int NC>
+__global__ void __launch_bounds__(128) k_fused_segment(DirP d, QueryP q, ChunkP ch, const uint32_t *list, uint32_t n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t seg = list ? list[i] : ch.seg_begin + i;
+    const size_t e = 2 * (size_t)(seg - ch.seg_begin);
+    const uint32_t rows = d.seg_rows[seg], series = d.seg_series[seg];
+    auto no_rows = [&]() { ch.edge_bucket[e] = OG_NO_BUCKET; ch.edge_bucket[e + 1] = OG_NO_BUCKET; };
+    if (d.seg_tmax[seg] < q.tmin || d.seg_tmin[seg] > q.tmax || rows == 0) { no_rows(); return; } /* segment pruning (location.go:276-280) */
+    const size_t ti_idx = (size_t)d.n_columns * d.n_segments + seg;
+    TimeDesc td;
+    int rc = parse_time_page(d.data + d.page_off[ti_idx], d.page_len[ti_idx], td);
+    if (rc != D_OK) { report_err(ch.err, rc, seg); no_rows(); return; }
+    TimeIter ti; ti.init(td);
+    ColIter col;
+    const size_t pi = (size_t)q.col_index[0] * d.n_segments + seg;
+    col.init(d.data + d.page_off[pi], d.page_len[pi], q.col_type[0], rows);
+    if (col.err != D_OK) { report_err(ch.err, col.err, seg); no_rows(); return; }
+    Part parts[NC];
+    uint32_t cur_b = OG_NO_BUCKET, head_b = OG_NO_BUCKET; bool head_done = false;
+    int64_t we = 0;
+    auto flush = [&](bool final) {
+        if (cur_b == OG_NO_BUCKET) return;
+#pragma unroll
+        for (int c = 0; c < NC; c++) {
+            if (!head_done) store_part(ch.edges[c], e, parts[c]);
+            else if (final) store_part(ch.edges[c], e + 1, parts[c]);
+            else if (parts[c].ok) store_cell(ch, (int)c, series, cur_b, parts[c]);
+        }
+        if (!head_done) { head_done = true; head_b = cur_b; }
+    };
+    uint32_t r = 0;
+    auto walk = [&](auto kind) {
+        col.kind = decltype(kind)::value; /* a constant from here on: value() reduces to this codec's case */
+        for (; r < rows; r++) {
+            const int64_t t = ti.next();
+            uint64_t v = 0;
+            const bool ok = col.next(v);
+            if (t < q.tmin) continue;
+            if (t > q.tmax) break;
+            if (cur_b == OG_NO_BUCKET || t >= we) {
+                flush(false);
+                cur_b = bucket_of(t, q.start, q.interval);
+                if (cur_b >= q.n_buckets) { report_err(ch.err, D_CORRUPT, seg); cur_b = OG_NO_BUCKET; break; } /* cannot happen on a validated shard */
+                we = q.start + (int64_t)(cur_b + 1) * q.interval;
+#pragma unroll
+                for (int c = 0; c < NC; c++) parts[c] = part_empty();
+            }
+            if (ok) {
+#pragma unroll
+                for (int c = 0; c < NC; c++) acc_row(q.calls[c].func, q.calls[c].type, parts[c], v, t);
+            }
+        }
+    };
+    using I = ColIter;
+    switch (col.kind) {
+    case I::K_ONE: walk(std::integral_constant<int, I::K_ONE>{}); break;
+    case I::K_F_RAW: walk(std::integral_constant<int, I::K_F_RAW>{}); break;
+    case I::K_F_GORILLA: walk(std::integral_constant<int, I::K_F_GORILLA>{}); break;
+    case I::K_F_SAME: walk(std::integral_constant<int, I::K_F_SAME>{}); break;
+    case I::K_F_RLE: walk(std::integral_constant<int, I::K_F_RLE>{}); break;
+    case I::K_I_CONST: walk(std::integral_constant<int, I::K_I_CONST>{}); break;
+    case I::K_I_S8B: walk(std::integral_constant<int, I::K_I_S8B>{}); break;
+    case I::K_I_RAW: walk(std::integral_constant<int, I::K_I_RAW>{}); break;
+    case I::K_B_BITS: walk(std::integral_constant<int, I::K_B_BITS>{}); break;
+    default: walk(std::integral_constant<int, I::K_ABSENT>{}); break; /* an all-null page (string columns never run here) */
+    }
+    if (r == rows) { /* the pages were walked to their last row (a scan that stops at tmax leaves the rest unread) */
+        ti.finish();
+        col.finish();
+    }
+    if (ti.err != D_OK) report_err(ch.err, ti.err, seg);
+    if (col.err != D_OK) report_err(ch.err, col.err, seg);
     const uint32_t last_b = cur_b;
     const bool single = !head_done;
     flush(true);

@@ -7,6 +7,7 @@ min/max/first/last and their times are still compared bitwise, float sums to 1e-
 run_both() runs every one-tagset query both ways.
 """
 import ctypes as C
+import struct
 
 import numpy as np
 import pytest
@@ -124,9 +125,11 @@ def test_decode_segment_matches_oracle():
     sh.close()
 
 
-def _one_segment_shard(typ, page, time_page, rows_t):
+def _one_segment_shard(typ, page, time_page, rows_t, n_cols=1):
+    """n_cols > 1: every column reads the same page"""
     data = np.concatenate([page, time_page])
-    return Shard.open(data, [1], [0, 1], [rows_t[0]], [rows_t[-1]], [("v", typ, [0], [page.size])], [page.size], [time_page.size])
+    cols = [(f"v{c}", typ, [0], [page.size]) for c in range(n_cols)]
+    return Shard.open(data, [1], [0, 1], [rows_t[0]], [rows_t[-1]], cols, [page.size], [time_page.size])
 
 
 @pytest.mark.parametrize("shape", ["raw", "same", "same0", "rle", "rle0", "gorilla", "gorilla_wrap", "one", "empty", "nulls"])
@@ -249,6 +252,106 @@ def test_unsupported_and_corrupt_pages_fail_cleanly():
     h = C.c_void_p()
     assert L.lib().og_query_create(sh.h, C.byref(d), C.byref(h)) == L.OG_E_INVAL
     sh.close()
+
+
+def _be(fmt, *v):
+    return np.frombuffer(struct.pack(">" + fmt, *v), np.uint8)
+
+
+def test_payload_that_disagrees_with_the_value_count(monkeypatch):
+    """Pages that pass og_shard_open but whose words / runs / bit stream do not hold the header's value count fail the same way
+    on every generic decode path; zero-length RLE runs of zeros pad nothing, zero-length runs of a value are corrupt.  A page whose
+    validity bitmap disagrees with its nil count is refused at og_shard_open."""
+    n = 100
+    t = T0 + np.arange(n, dtype=np.int64) * SEC
+    tp = oracle.time_page_encode(t)
+    ipage = oracle.field_page_encode(L.TYPE_INT, np.cumsum(np.random.default_rng(2).integers(-1000, 1001, n)).astype(np.int64))
+    assert ipage[5] >> 4 == 2  # Full header (5 B), then [tag][u32 encCount][u32 srcCount][u64 first][encCount - 1 words]
+    enc = struct.unpack(">I", ipage[6:10].tobytes())[0]
+    assert ipage.size == 14 + 8 * enc
+    surplus = np.concatenate([ipage[:6], _be("I", enc + 1), ipage[10:], _be("Q", 0xF << 60)])  # one more word: selector 15, one value
+    missing = np.concatenate([ipage[:6], _be("I", enc - 1), ipage[10:-8]])
+    fpage = oracle.field_page_encode(L.TYPE_FLOAT, np.repeat([1.5, 2.5, 0.0, 7.0], n // 4))
+    assert fpage[5] >> 4 == 5  # RLE: runs of [u16 BE count (bit 15: zero run)][8 B LE value]
+    run0 = struct.unpack(">H", fpage[6:8].tobytes())[0]
+    rle_n1 = np.concatenate([fpage[:6], _be("H", run0 + 1), fpage[8:]])
+    rle_zero0 = np.concatenate([fpage[:6], _be("H", 0x8000), fpage[6:]])
+    rle_value0 = np.concatenate([fpage[:6], _be("H", 0), np.full(8, 0x11, np.uint8), fpage[6:]])
+    gpage = oracle.field_page_encode(L.TYPE_FLOAT, 100 + np.random.default_rng(3).random(n))
+    assert gpage[5] >> 4 == 3  # Gorilla: [tag][0x10][8 B first][bit stream]
+    gorilla_cut = gpage[:15 + (gpage.size - 15) // 2]  # half the bit stream
+
+    def paths(typ, page):
+        """(label, run) for og_decode_segment, path 1, path 0 and path 4; run() returns the dense result of the aggregates"""
+        sh = _one_segment_shard(typ, page, tp, t, n_cols=2)
+
+        def query(calls, flags, path):
+            q = AggQuery(sh, calls, 0, int(t[0]), int(t[-1]), flags=flags)
+            try:
+                q.run()
+                assert q.stats()["path"] == path
+                return q.dense_host()
+            finally:
+                q.close()
+
+        def multi():
+            with monkeypatch.context() as m:
+                m.setenv("OGPU_NO_COLS", "1")
+                return query([("sum", 0), ("count", 1), ("max", 0)], 0, 4)
+        return sh, [("decode", lambda: sh.decode_segment(0)),
+                    ("path 1", lambda: query([("sum", 0), ("count", 0), ("max", 0)], L.Q_NO_FAST, 1)),
+                    ("path 0", lambda: query([("sum", 0), ("count", 0), ("max", 0)], L.Q_NO_FUSED, 0)),
+                    ("path 4", multi)]
+
+    for label, typ, page in (("s8b surplus word", L.TYPE_INT, surplus), ("s8b missing word", L.TYPE_INT, missing),
+                             ("rle n+1", L.TYPE_FLOAT, rle_n1), ("rle zero-length value run", L.TYPE_FLOAT, rle_value0),
+                             ("truncated gorilla", L.TYPE_FLOAT, gorilla_cut)):
+        sh, runs = paths(typ, page)
+        for where, run in runs:
+            with pytest.raises(L.OgpuError) as ei:
+                run()
+            assert ei.value.status == L.OG_E_CORRUPT, f"{label}, {where}"
+        sh.close()
+
+    want, _ = oracle.field_page_decode(L.TYPE_FLOAT, rle_zero0)
+    assert want.size == n
+    s = 0.0
+    for x in want:
+        s += x
+    sh, runs = paths(L.TYPE_FLOAT, rle_zero0)
+    for where, run in runs:
+        got = run()
+        if where == "decode":
+            assert np.array_equal(got["cols"][0]["values"].view(np.uint64), want.view(np.uint64)), where
+            continue
+        vals = [got["cols"][k]["values"][0] for k in range(3)]
+        assert all(got["cols"][k]["valid"][0] for k in range(3)), where
+        assert (float(vals[0]), int(vals[1]), float(vals[2])) == (s, n, want.max()), where
+    sh.close()
+
+    # a Simple8b time page with a missing word is refused when the shard is opened
+    ti = T0 + np.cumsum(np.random.default_rng(4).integers(1, 5000, n)).astype(np.int64)
+    tpage = oracle.time_page_encode(ti)
+    assert tpage[5] >> 4 == 2  # [tag][u64 scale][u32 encCount][u32 srcCount][u64 first][encCount - 1 words]
+    tenc = struct.unpack(">I", tpage[14:18].tobytes())[0]
+    assert tpage.size == 22 + 8 * tenc
+    tbad = np.concatenate([tpage[:14], _be("I", tenc - 1), tpage[18:-8]])
+    with pytest.raises(L.OgpuError) as ei:
+        _one_segment_shard(L.TYPE_FLOAT, oracle.field_page_encode(L.TYPE_FLOAT, 100 + np.zeros(n)), tbad, ti)
+    assert ei.value.status == L.OG_E_CORRUPT
+
+    # a bitmap that marks one row more valid than the header's value count is refused when the shard is opened
+    valid = np.ones(n, np.uint8); valid[[3, 50]] = 0
+    npage = oracle.field_page_encode(L.TYPE_FLOAT, 100 + np.random.default_rng(5).random(n), valid)
+    assert npage[0] == L.TYPE_FLOAT  # normal header: [type][u32 bitmap bytes][bitmap][u32 bitmap offset][u32 nil count][block]
+    nb = struct.unpack(">I", npage[1:5].tobytes())[0]
+    nil = struct.unpack(">I", npage[9 + nb:13 + nb].tobytes())[0]
+    assert nil == 2
+    bad = np.concatenate([npage[:9 + nb], _be("I", nil + 1), npage[13 + nb:]])
+    _one_segment_shard(L.TYPE_FLOAT, npage, tp, t).close()
+    with pytest.raises(L.OgpuError) as ei:
+        _one_segment_shard(L.TYPE_FLOAT, bad, tp, t)
+    assert ei.value.status == L.OG_E_CORRUPT
 
 
 # ---------------------------------------------------------------------------------------------------------------
