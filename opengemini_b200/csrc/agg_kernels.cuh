@@ -40,13 +40,17 @@ struct ChunkP { /* one chunk of whole series */
     uint32_t nb;                       /* buckets per series row (= QueryP.n_buckets) */
     Tri edges[OG_MAX_CALLS];           /* [ 2 * (seg - seg_begin) + {0 head, 1 tail} ] */
     uint32_t *edge_bucket;             /* [ 2 * (seg - seg_begin) ] OG_NO_BUCKET = absent */
-    Tri gcells[OG_MAX_CALLS];          /* folded window partials [ b * gc_cols + col ] (one tagset, regular shard): col < gc_edge0 is a
-                                          lane group of the fused kernel (32 series folded in-warp), col >= gc_edge0 a block of 32
-                                          consecutive series whose stitched edge windows k_fix_edges_fold folded.  nullptr when unused */
-    uint32_t gc_cols, gc_edge0, gc_col0;
+    Tri gcells[OG_MAX_CALLS];          /* folded window partials [ b * gc_cols + col ] (one tagset, regular shard): col < gc_tail0 is a
+                                          lane group of the fused kernel (32 series folded in-warp: interior and head windows),
+                                          gc_tail0 + col the tail windows of that lane group, col >= gc_edge0 a block of 32
+                                          consecutive series whose stitched edge windows k_fix_edges_fold folded (three blocks of
+                                          columns: runs led by a head window of even / odd segment index, runs led by a tail
+                                          window).  nullptr when unused */
+    uint32_t gc_cols, gc_tail0, gc_edge0, gc_col0;
     uint32_t J;                        /* segments per series on a regular shard, else 0 */
     int *err;                          /* [0] first error code, [1] segment */
-    int *flags;                        /* [0] != 0: some kernel wrote per-series cells in this run (the cell merges have work) */
+    int *flags;                        /* [0] != 0: some kernel wrote per-series cells in this run (the cell merges have work);
+                                          [1] != 0: k_fused_il or k_fused_segment wrote edge windows (k_fix_edges_fold has work) */
 };
 
 __device__ __forceinline__ size_t cell_idx(const ChunkP &ch, uint32_t series, uint32_t b) { return (size_t)(series - ch.series_begin) * ch.nb + b; }
@@ -351,9 +355,11 @@ __device__ __forceinline__ bool call_has_time(const QueryP &q, uint32_t c) { ret
 __device__ __forceinline__ int call_ftype(const QueryP &q, uint32_t c) { return q.calls[c].func == OG_AGG_COUNT ? OG_TYPE_INT : q.calls[c].type; }
 
 /* regular shards, one tagset: warp per (block of 32 consecutive series, segment index); the lanes' stitched windows of one
- * bucket are folded in-warp into ONE cell of the folded matrix (column gc_edge0 + block).  Blocks whose series do not agree
- * on the bucket (irregular time grids) fall back to per-series cells. */
+ * bucket are folded in-warp into ONE cell of the folded matrix (a column of the block).  Blocks whose series do not agree
+ * on the bucket (irregular time grids) fall back to per-series cells.  Segments whose edge windows k_fused_il folded in the warp
+ * have no edge_bucket entries; when no kernel of this chunk wrote an edge window the launch returns at once. */
 __global__ void k_fix_edges_fold(DirP d, QueryP q, ChunkP ch) {
+    if (ch.flags[1] == 0) return;
     const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     const uint32_t n_blk = (ch.series_end - ch.series_begin + 31) / 32;
     if (w >= n_blk * ch.J) return;
@@ -363,8 +369,19 @@ __global__ void k_fix_edges_fold(DirP d, QueryP q, ChunkP ch) {
     const uint32_t seg = in ? d.series_seg_begin[series] + j : 0;
     EdgeRuns r; r.hb = r.tb = OG_NO_BUCKET; r.head_leader = false; r.s_end = 0;
     if (in) r = edge_runs(d, ch, seg, series);
-    const uint32_t gcol = ch.gc_edge0 + ch.series_begin / 32 + blk - ch.gc_col0;
+    /* Every warp of a block stores with plain stores, so two warps of one block (two segment indices) must never write the
+     * same (bucket, column).  Once some segments fold their edges in k_fused_il, the run of a bucket X may be led by different
+     * segment indices in different series of the block: by tail(j) in a series whose segment j is stitched, by head(j+1) in
+     * one whose segment j was folded; and by head(j) in a series whose segment j starts in X (a range that cuts segment j,
+     * a coarser cadence) next to head(j+1) in one whose segment j was folded with its tail in X.  Hence three columns per
+     * block: runs led by a tail window, and runs led by a head window of even and of odd j.  That suffices on the shards
+     * the plan folds (segment index j covers one [seg_tmin, seg_tmax] in every series): tails of one bucket all come from
+     * one j (times ascend with j), and heads from at most j and j+1 — if a series had a head-led run at X from j and another
+     * one from j+2, segment j+1 would lie wholly inside X in both, and in the second series it would carry the run into j+2
+     * (its last edge window is X, so head(j+2) does not lead). */
+    const uint32_t n_bk = (ch.gc_cols - ch.gc_edge0) / 3;
     for (int which = 0; which < 2; which++) {
+        const uint32_t gcol = ch.gc_edge0 + (which ? 2u : (j & 1u)) * n_bk + ch.series_begin / 32 + blk - ch.gc_col0;
         const bool has = r.hb != OG_NO_BUCKET && (which == 0 ? r.head_leader : r.tb != OG_NO_BUCKET);
         const uint32_t b = which == 0 ? r.hb : r.tb;
         const uint32_t hm = __ballot_sync(0xffffffffu, has);

@@ -540,7 +540,9 @@ int ensure_il(og_shard *s, int col, cudaStream_t st) {
     if ((rc = tmp.get(&seg_words, nseg)) || (rc = tmp.get(&so.seg_t0, nseg)) || (rc = tmp.get(&so.seg_dt, nseg)) || (rc = tmp.get(&so.keys, nseg)) ||
         (rc = tmp.get(&so.vals, nseg)) || (rc = tmp.get(&keys2, nseg)) || (rc = tmp.get(&vals2, nseg)) || (rc = tmp.get(&so.dom_cnt, n_dom))) return rc;
     so.seg_words = seg_words;
+    if ((rc = tmp.get(&so.misaligned, 1))) return rc;
     CU(cudaMemsetAsync(so.dom_cnt, 0, (size_t)n_dom * 4, st));
+    CU(cudaMemsetAsync(so.misaligned, 0, 4, st));
     DirP d = make_dir(s);
     k_il_scan<<<(nseg + 255) / 256, 256, 0, st>>>(d, col, s->col_types[col], J, so);
     CU(cudaGetLastError());
@@ -552,8 +554,9 @@ int ensure_il(og_shard *s, int col, cudaStream_t st) {
         void *dtmp; if ((rc = tmp.get((uint8_t **)&dtmp, tb))) return rc;
         CU(cub::DeviceRadixSort::SortPairs(dtmp, tb, so.keys, keys2, so.vals, vals2, (int)nseg, 0, (int)OG_IL_WORD_BITS + dbits, st));
     }
-    std::vector<uint32_t> dom_cnt(n_dom);
+    std::vector<uint32_t> dom_cnt(n_dom); uint32_t misaligned = 1;
     CU(cudaMemcpyAsync(dom_cnt.data(), so.dom_cnt, (size_t)n_dom * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&misaligned, so.misaligned, 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     std::vector<uint32_t> elem_first(n_dom), grp_first(n_dom);
     uint64_t n_elig = 0, ng64 = 0;
@@ -569,7 +572,7 @@ int ensure_il(og_shard *s, int col, cudaStream_t st) {
     }
     if (n_elig == 0) return OG_OK;
     const uint32_t ng = (uint32_t)ng64;
-    ic.n_groups = ng; ic.J = J; ic.n_super = n_super; ic.cols_per_super = OG_IL_SUPER / 32 + 1;
+    ic.n_groups = ng; ic.J = J; ic.aligned = J != 0 && misaligned == 0; ic.n_super = n_super; ic.cols_per_super = OG_IL_SUPER / 32 + 1;
     ic.super_grp_first.assign(n_super + 1, ng);
     for (uint32_t sp = 0; sp < n_super; sp++) ic.super_grp_first[sp] = grp_first[J ? sp * J : 0];
     uint32_t *d_elem_first, *d_grp_first;
@@ -672,7 +675,9 @@ int build_plan(og_query *q) {
     pl->fast = want_fast && s->il[p.col_index[0]].state == 1;
     const og_shard::IlCol *ic = pl->fast ? &s->il[p.col_index[0]] : nullptr;
     pl->ic = ic;
-    pl->fold = pl->fast && ic->J != 0 && q->desc.group_mode == OG_GROUP_ALL && !(q->desc.flags & OG_Q_STRICT_ORDER);
+    /* folding needs every segment index of a binning domain to cover one time range: lane groups of one rank share a column of
+     * the folded matrix across segment indices (k_il_assign), and their cells must land in distinct buckets */
+    pl->fold = pl->fast && ic->J != 0 && ic->aligned && q->desc.group_mode == OG_GROUP_ALL && !(q->desc.flags & OG_Q_STRICT_ORDER);
 
     /* chunk plan: whole series per chunk, per-series cells bounded by a memory budget */
     size_t cell_bytes_per_series = 0;
@@ -723,9 +728,10 @@ int build_plan(og_query *q) {
             if (sel && (rc = salloc(q, &ch.gcells[c].tim, n))) return rc;
         }
     }
-    if (pl->fold) { /* folded cell matrix: lane-group columns, then one column per block of 32 consecutive series (stitched edge windows) */
-        ch.gc_edge0 = ic->n_super * ic->cols_per_super; ch.gc_col0 = 0;
-        ch.gc_cols = ch.gc_edge0 + (s->n_series + 31) / 32;
+    if (pl->fold) { /* folded cell matrix: lane-group columns, their tail-window columns, then three columns per block of 32 consecutive
+                       series (stitched edge windows: runs led by a head window of even / odd segment index, runs led by a tail window) */
+        ch.gc_tail0 = ic->n_super * ic->cols_per_super; ch.gc_edge0 = 2 * ch.gc_tail0; ch.gc_col0 = 0;
+        ch.gc_cols = ch.gc_edge0 + 3 * ((s->n_series + 31) / 32);
         const size_t n = (size_t)p.n_buckets * ch.gc_cols;
         for (uint32_t c = 0; c < p.n_calls; c++) {
             bool sel = p.calls[c].func >= OG_AGG_MIN;
@@ -814,6 +820,7 @@ OG_API int og_query_run(og_query *q) {
         if (clear_cells) for (uint32_t c = 0; c < p.n_calls; c++) CU(cudaMemsetAsync(ch.cells[c].ok, 0, chunk_cells, st));
         /* folded cells are per chunk: a lane group that straddles chunks contributes to its column once per chunk */
         if (pl->fold || pl->blockmerge) for (uint32_t c = 0; c < p.n_calls; c++) CU(cudaMemsetAsync(ch.gcells[c].ok, 0, (size_t)p.n_buckets * ch.gc_cols, st));
+        if (pl->fold && ci > 0) CU(cudaMemsetAsync(ch.flags + 1, 0, sizeof(int), st)); /* "edge windows written" is per chunk (the run's first chunk starts from the cleared error buffer) */
         CU(cudaEventRecord(q->main_ev[2 * chunks_run], st));
         if (pl->fused) {
             const uint32_t *gl = nullptr; uint32_t gn = nseg;
@@ -875,10 +882,13 @@ OG_API int og_query_run(og_query *q) {
     int err[16];
     CU(cudaMemcpy(err, q->d_err, 64, cudaMemcpyDeviceToHost));
     if (getenv("OGPU_IL_STATS")) {
-        unsigned long long wait, life; /* warp cycles waiting for ring batches / over the warp's lifetime (OG_IL_STATS builds) */
-        memcpy(&wait, err + 8, 8); memcpy(&life, err + 10, 8);
-        fprintf(stderr, "[ogpu] fused rounds: common %d rare %d (lanes not resident in %d, sit-outs %d); warp cycles: %llu waiting for batches of %llu (%.1f %%)\n",
-                err[4], err[5], err[6], err[7], wait, life, life ? 100.0 * (double)wait / (double)life : 0.0);
+        /* warp cycles waiting for ring batches / over the warp's lifetime / before the first round / after the last round (OG_IL_STATS builds) */
+        unsigned long long wait, life, pro, epi;
+        memcpy(&wait, err + 8, 8); memcpy(&life, err + 10, 8); memcpy(&pro, err + 12, 8); memcpy(&epi, err + 14, 8);
+        const double pc = life ? 100.0 / (double)life : 0.0;
+        fprintf(stderr, "[ogpu] fused rounds: common %d rare %d (lanes not resident in %d, sit-outs %d); warp cycles: %llu waiting for batches of %llu (%.1f %%), "
+                "prologue %llu (%.1f %%), epilogue %llu (%.1f %%)\n",
+                err[4], err[5], err[6], err[7], wait, life, pc * (double)wait, pro, pc * (double)pro, epi, pc * (double)epi);
     }
     q->cells_dirty = err[2] != 0;
     if (err[0]) { set_error("segment %d failed to decode (device code %d)", err[1], err[0]); return map_dev_err(err[0]); }

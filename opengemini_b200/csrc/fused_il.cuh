@@ -24,11 +24,13 @@
  *             Raw pages are transcoded by the repack into fixed 64-bit XOR deltas, which the same path decodes with
  *             MASK = ~0 and no control bits — there is no separate raw-page kernel.
  *   reduce    window boundaries are row countdowns derived from the const-delta time page; rounds in which no lane reaches
- *             a boundary run without the per-record test.  Partials stay in registers.  First/last window of a segment go
- *             to the edge arrays (k_fix_edges stitches them across segments).  Interior windows: when the query has one
- *             tagset and the lanes share a time grid, the 32 partials of a bucket are folded with warp shuffles and ONE
- *             cell per (bucket, group) is written (gcells; 32x fewer cells, no per-series cell traffic); otherwise each
- *             lane writes its own cell (cells[series][bucket]) and the fold happens in k_merge_* in strict series order.
+ *             a boundary run without the per-record test.  Partials stay in registers.  When the query has one tagset and
+ *             the lanes share a time grid, the 32 partials of a bucket are folded with warp shuffles and ONE cell per
+ *             (bucket, group) is written (gcells; 32x fewer cells, no per-series cell traffic) — interior windows and, when
+ *             the group spans more than one bucket, the first/last window of its segments too (tail windows in a column of
+ *             their own).  Otherwise the first/last window of a segment goes to the edge arrays (k_fix_edges stitches them
+ *             across segments) and each lane writes its own interior cells (cells[series][bucket]), folded in k_merge_* in
+ *             strict series order.
  *
  * Replaces for eligible segments: tsm1.FloatArrayDecodeAll (batch_float.go:278-514) + Time.constDeltaDecoding
  * (timestamp.go:190) + FilterByTime (reader.go:754) + getIntervalIndex/reduce (aggregate_cursor.go:306-356) +
@@ -203,7 +205,7 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
         r_lo = 0; r_hi = rows - 1;
         if (t0 < q.tmin) { uint64_t k = udiv_est((uint64_t)(q.tmin - t0) + dtu - 1, dtu, inv_dt); r_lo = k > rows ? rows : (uint32_t)k; }
         { int64_t t_last = t0 + (int64_t)(rows - 1) * dt; if (t_last > q.tmax) { if (q.tmax < t0) r_lo = rows; else r_hi = (uint32_t)udiv_est((uint64_t)(q.tmax - t0), dtu, inv_dt); } }
-        if (r_lo > r_hi || r_lo >= rows) { ch.edge_bucket[e] = OG_NO_BUCKET; ch.edge_bucket[e + 1] = OG_NO_BUCKET; active = false; }
+        if (r_lo > r_hi || r_lo >= rows) { *(uint2 *)(ch.edge_bucket + e) = make_uint2(OG_NO_BUCKET, OG_NO_BUCKET); active = false; }
     }
     if (!__any_sync(FULL, active)) return;
 
@@ -267,8 +269,22 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
      * them and the segment spans at most WCAP of them.  Lanes may still reach a window at different moments (streams of different
      * entropy drift apart): interior windows are therefore accumulated per bucket in shared memory — whoever closes a window adds
      * its partial, lanes that close the same window in the same step are folded with shuffles first — and written to the folded
-     * cell matrix once, when the whole group is done. ---- */
-    bool uni = false; uint32_t b0 = 0;
+     * cell matrix once, when the whole group is done.
+     *
+     * Edge windows: the first and last window of a segment may continue in the neighbouring segments of its series.  When the
+     * group's rows span more than one bucket (b_end > b0), the lanes' head windows all lie in bucket b0 and their tail windows
+     * all in b_end, so they are accumulated like interior windows: the head in column gcol (slot 0), the tail in the group's
+     * TAIL column gc_tail0 + gcol (slot b_end - b0).  Tails need columns of their own: group (j, r) has its tail in the bucket
+     * of the head of group (j+1, r), same column r.  Heads (and tails) of one column never meet in a bucket because segment
+     * index j covers one time range in every series of the binning domain (the plan folds only such shards) and those ranges
+     * are disjoint and ascending in j: tail(j) <= head(j+1) < tail(j+1).  A group inside one bucket (a window spanning three or
+     * more segments) and groups whose lanes disagree (uni false) write their edges to ch.edges for k_fix_edges_fold, and flag
+     * it.  Mixing the two is exact: a segment folded here has no edge_bucket entries, which the stitch reads as "no rows in
+     * range", so its neighbour leads a run of its own and the two partials of the bucket meet in k_merge_folded through
+     * group_update.  Count, sum, min and max are associative there; for selectors that carry a time the part of a series in
+     * its tail (earlier times) and the part in the next segment's head (later times) are ordered by time, and group_update
+     * picks the earlier time on equal values (first/last: the earlier/later time), exactly what the ordered stitch picks. ---- */
+    bool uni = false; uint32_t b0 = 0, b_end = 0;
     uint64_t *acc_v = nullptr; int64_t *acc_t = nullptr; uint8_t *acc_k = nullptr;
     if (FOLD) {
         const int leader = __ffs(__ballot_sync(FULL, active)) - 1;
@@ -280,6 +296,7 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
         const uint32_t b_last = active ? (uint32_t)udiv_est((uint64_t)(t0 + (int64_t)r_hi * dt - q.start), (uint64_t)q.interval, inv_iv) : b0;
         uni = __all_sync(FULL, !active || (same && b_last - b0 < OG_IL_WCAP));
         if (uni) {
+            b_end = __reduce_max_sync(FULL, active ? b_last : 0u);
             const uint32_t nacc = OG_IL_WCAP * q.n_calls;
             uint8_t *base = s_acc + (size_t)wid * il_acc_bytes(q.n_calls, TIMES);
             acc_v = (uint64_t *)base; acc_t = (int64_t *)(base + (size_t)nacc * 8); acc_k = base + (size_t)nacc * (TIMES ? 16 : 8);
@@ -288,6 +305,8 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
         }
     }
     const uint32_t gcol = FOLD ? il.grp_col[grp] - ch.gc_col0 : 0;
+    /* edge windows folded in the warp as well (head in slot 0, tail in slot b_end - b0; see "edge windows" above) */
+    const bool fold_edges = FOLD && uni && b_end > b0;
 
     /* ---- per-window partials ---- */
     double sum = 0.0, mn = 0.0, mx = 0.0; uint64_t fi = 0, lastv = 0;
@@ -463,6 +482,7 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
     uint32_t rounds_left = hung ? 0u : 40u * (__reduce_max_sync(FULL, rows) / K + 8u);
 #ifdef OG_IL_STATS
     uint32_t st_common = 0, st_rare = 0, st_sit = 0, st_notgo = 0;
+    const long long st_pro = clock64() - st_clk0; /* prologue: warp start to the first round (metadata chain, first batch) */
 #endif
     for (;;) {
         const uint32_t qmin = __reduce_min_sync(FULL, done ? 0xffffffffu : qp);
@@ -525,8 +545,10 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
             if (FOLD && uni) {
                 const bool fl = ev && !skipping;
                 const int kind = kind_of();
-                if (fl && kind != 2) flush_lane(kind);
-                if (__any_sync(FULL, fl && kind == 2)) flush_fold(fl && kind == 2);
+                const bool to_acc = fl && (kind == 2 || fold_edges);
+                if (fl && !to_acc) flush_lane(kind);
+                if (__any_sync(FULL, to_acc)) flush_fold(to_acc);
+                if (to_acc && kind == 0) head_done = true;
             } else if (ev && !skipping) flush_lane(kind_of());
             if (ev) advance();
             /* every live lane crossed a window boundary in the same step (lanes that share a time grid always do): start a fresh
@@ -537,29 +559,35 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
     }
     if (active && (qp >> 5) >= rows_w) bad = 1; /* ran past the stream: corrupt page */
 #ifdef OG_IL_STATS
+    const long long st_e0 = clock64(); /* epilogue: last round to warp end (drain, cell and edge stores) */
     if (lane == 0) { atomicAdd((unsigned *)&ch.err[4], st_common); atomicAdd((unsigned *)&ch.err[5], st_rare); atomicAdd((unsigned *)&ch.err[6], st_notgo); atomicAdd((unsigned *)&ch.err[7], st_sit); }
 #endif
     /* copies still in flight must land before this CTA's shared memory can be reused */
     while (ready_b < issued_b && hung != 1) { if (!mbar_wait(bar0 + (ready_b % NB) * 8, (ready_b / NB) & 1)) hung = 1; ready_b++; }
     if (hung && lane == 0) report_err(ch.err, D_WATCHDOG, (grp << 2) | hung);
-    if (FOLD && uni) { /* the group's interior windows -> one cell per bucket */
+    if (FOLD && uni) { /* the group's folded windows -> one cell per bucket (the tail window to the tail column) */
         __syncwarp();
+        const uint32_t w_tail = fold_edges ? b_end - b0 : OG_IL_WCAP;
         for (uint32_t i = lane; i < OG_IL_WCAP * q.n_calls; i += 32) {
             if (!acc_k[i]) continue;
             const uint32_t c = i / OG_IL_WCAP, w = i % OG_IL_WCAP;
             Part a; a.ok = 1; a.v = acc_v[i]; a.t = TIMES ? acc_t[i] : 0;
-            store_part(ch.gcells[c], (size_t)(b0 + w) * ch.gc_cols + gcol, a);
+            store_part(ch.gcells[c], (size_t)(b0 + w) * ch.gc_cols + (w == w_tail ? ch.gc_tail0 + gcol : gcol), a);
         }
     }
+    /* some lane wrote edge windows: k_fix_edges_fold has work */
+    if (FOLD && __any_sync(FULL, active && head_b != OG_NO_BUCKET) && lane == 0) ch.flags[1] = 1;
     if (active) {
         if (bad) report_err(ch.err, D_CORRUPT, seg);
-        ch.edge_bucket[e] = head_b;
-        ch.edge_bucket[e + 1] = (head_b == OG_NO_BUCKET || cur_b == head_b) ? OG_NO_BUCKET : cur_b;
+        *(uint2 *)(ch.edge_bucket + e) = make_uint2(head_b, (head_b == OG_NO_BUCKET || cur_b == head_b) ? OG_NO_BUCKET : cur_b);
     }
 #ifdef OG_IL_STATS
     if (lane == 0) {
         atomicAdd((unsigned long long *)(ch.err + 8), (unsigned long long)st_wait);
-        atomicAdd((unsigned long long *)(ch.err + 10), (unsigned long long)(clock64() - st_clk0));
+        const long long st_end = clock64();
+        atomicAdd((unsigned long long *)(ch.err + 10), (unsigned long long)(st_end - st_clk0));
+        atomicAdd((unsigned long long *)(ch.err + 12), (unsigned long long)st_pro);
+        atomicAdd((unsigned long long *)(ch.err + 14), (unsigned long long)(st_end - st_e0));
     }
 #endif
 }

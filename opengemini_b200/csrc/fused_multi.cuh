@@ -212,6 +212,7 @@ __global__ void __launch_bounds__(128) k_fused_segment(DirP d, QueryP q, ChunkP 
     flush(true);
     ch.edge_bucket[e] = head_b;
     ch.edge_bucket[e + 1] = (single || head_b == OG_NO_BUCKET) ? OG_NO_BUCKET : last_b;
+    if (head_b != OG_NO_BUCKET) ch.flags[1] = 1; /* edge windows written: k_fix_edges_fold has work */
 }
 
 } // namespace ogpu

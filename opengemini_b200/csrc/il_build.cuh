@@ -5,7 +5,8 @@
  *                    const-delta time page's (t0, dt), and the sort key (domain, words).  A domain is the set of segments that
  *                    may share a lane group: on regular shards (every series has J segments) segment index j of a block of
  *                    OG_IL_SUPER consecutive series — they cover the same time range, so their windows coincide; otherwise
- *                    the whole shard.
+ *                    the whole shard.  It also checks that every segment index covers one [seg_tmin, seg_tmax] across the
+ *                    series of its domain (the folded query path relies on it).
  *   radix sort       (cub::DeviceRadixSort, stable) orders the eligible segments by (domain, words): 32 consecutive entries of
  *                    one domain make a lane group of similar stream lengths.
  *   k_il_assign      sorted position -> (group, lane) slot; writes the per-lane metadata the kernel needs (segment, rows,
@@ -31,6 +32,7 @@ struct IlScanOut {
     uint64_t *keys;         /* [n_segments] sort key, ~0 = not eligible */
     uint32_t *vals;         /* [n_segments] = segment id */
     uint32_t *dom_cnt;      /* [n_domains] eligible segments per domain */
+    uint32_t *misaligned;   /* [1] set when some segment index covers different time ranges in two series of one domain */
 };
 
 __global__ void k_il_scan(DirP d, int col, int col_type, uint32_t J, IlScanOut o) {
@@ -57,8 +59,12 @@ __global__ void k_il_scan(DirP d, int col, int col_type, uint32_t J, IlScanOut o
         }
     }
     o.ok[seg] = c; o.seg_words[seg] = nw; o.seg_t0[seg] = t0; o.seg_dt[seg] = dt; o.vals[seg] = seg;
-    if (c == SEG_GENERAL) { o.keys[seg] = ~0ull; return; }
     const uint32_t series = d.seg_series[seg];
+    if (J) { /* same time range as segment index j of the domain's first series? */
+        const uint32_t ref = d.series_seg_begin[series / OG_IL_SUPER * OG_IL_SUPER] + (seg - d.series_seg_begin[series]);
+        if (d.seg_tmin[seg] != d.seg_tmin[ref] || d.seg_tmax[seg] != d.seg_tmax[ref]) *o.misaligned = 1;
+    }
+    if (c == SEG_GENERAL) { o.keys[seg] = ~0ull; return; }
     const uint32_t dom = J ? (series / OG_IL_SUPER) * J + (seg - d.series_seg_begin[series]) : 0u;
     o.keys[seg] = ((uint64_t)dom << OG_IL_WORD_BITS) | nw;
     atomicAdd(&o.dom_cnt[dom], 1u);

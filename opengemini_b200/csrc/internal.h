@@ -68,6 +68,7 @@ struct og_shard {
                    uint32_t *lane_seg = nullptr, *lane_rows = nullptr, *lane_series = nullptr; int64_t *lane_t0 = nullptr; uint64_t *lane_dt = nullptr;
                    uint32_t *gen_list = nullptr; std::vector<uint32_t> gen_host; /* segments the fused kernel does not take (ascending), device + host */
                    uint32_t n_groups = 0, J = 0; /* J != 0: regular shard, lane groups share a segment index */
+                   bool aligned = false; /* regular shard whose segment index j has one [seg_tmin, seg_tmax] in every series of a binning domain */
                    uint32_t n_super = 1, cols_per_super = 0; std::vector<uint32_t> super_grp_first; /* [n_super+1] first lane group of each block of OG_IL_SUPER series */
                    uint64_t n_words = 0; double build_ms = 0; };
     std::vector<IlCol> il; /* [n_columns] */
