@@ -8,6 +8,8 @@
  *                            ChunkMeta.colMeta[i].entries[seg]{offset,size}, tssp_file_meta.go:60-63,377-385)
  *                            + lib/fileops/readcache page access.  Here: one upload of the data region + the
  *                            flattened ChunkMeta ("segment directory") into HBM.
+ *   og_shard_open_files      the per-query merge of a shard's ordered and out-of-order files (engine/iterators.go:246,295,
+ *                            agg_tagset_cursor.go:294-346,411-535, iterators_helper.go:484 mergeData), done once at open.
  *   og_tssp_parse/_desc      the directory half of the file open: footer -> trailer -> meta index -> chunk-meta blocks ->
  *                            ChunkMeta (engine/immutable/trailer.go:71-88, tssp_file_meta.go:606-687,789-802,
  *                            tssp_file.go:606-658); yields the og_shard_desc og_shard_open takes.  Host only.
@@ -254,6 +256,39 @@ OG_API int og_shard_open(const og_shard_desc *desc, og_shard **out);
 OG_API void og_shard_close(og_shard *s);
 OG_API int og_shard_info(const og_shard *s, uint64_t *n_series, uint64_t *n_segments, uint64_t *n_rows,
                          uint64_t *page_bytes, int64_t *tmin, int64_t *tmax);
+
+/* ---- a shard's ordered and out-of-order files as ONE og_shard (csrc/merge.cu).  Replaces the per-query file-set read of the
+ * reference: ordered files visited one after another (engine/agg_tagset_cursor.go:294-346), out-of-order files merged newest
+ * first (agg_tagset_cursor.go:411-535, MergeRecordLimitRows), the result merged into the ordered records (engine/file_cursor.go:
+ * 292-348 -> iterators_helper.go:484 mergeData -> lib/record/record.go:843 MergeRecordByMaxTimeOfOldRec), over the files that
+ * immTables.GetBothFilesRef hands a query (engine/iterators.go:246,295).  Here the merge runs once, on the device, when the shard
+ * is opened, and every query / decode / downsample / export entry point serves the result.
+ *   files[]      in file-sequence order, oldest first (ordered and out-of-order files interleaved as they come); each is what
+ *                og_tssp_desc or a caller builds for og_shard_open, with host data (OG_SHARD_DEVICE_DATA is refused here).
+ *   file_flags[] OG_FILE_OUT_OF_ORDER marks the out-of-order files; every out-of-order file is newer than every ordered one.
+ * Row rule (record.go:468-505 mergeRecRow): where files hold the same series and time, each column takes the newest file's value,
+ * the older one's when that is null.  The schema is the union of the field columns by name, sorted by name (record.go:438-466); a
+ * column a file lacks is null for its rows.  Series are the union by sid, ascending.
+ * Only the rows of a series around its out-of-order rows are re-encoded (1000-row segments, the encoders of og_encode_pages; a
+ * float segment the Gorilla encoder refuses gets a raw page): ordered segments outside that span keep their bytes.
+ * Refused: a column with two types (OG_E_TYPE), ordered files that overlap in time for one series, a string column with values
+ * inside a re-encoded span (OG_E_UNSUPPORTED), a time repeated within one file's series inside a span (OG_E_CORRUPT).
+ * WHERE applies to the merged row (the reference filters each file before the merge: DESIGN.md "Deviations"). ---- */
+enum { OG_FILE_OUT_OF_ORDER = 1u << 0 };
+OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, og_shard **out);
+typedef struct og_merge_info {
+    uint32_t n_files, n_out_of_order_files;
+    uint64_t series_merged;          /* series that had out-of-order rows */
+    uint64_t out_of_order_rows;      /* rows read from out-of-order files */
+    uint64_t rows_replaced;          /* older rows whose time a newer file also holds */
+    uint64_t rows_after_merge;
+    uint64_t segments_kept;          /* ordered segments carried over byte for byte */
+    uint64_t segments_rewritten_in, segments_rewritten_out;
+    double merge_ms;                 /* elapsed time of the merge phase, from the first batch to the assembled data region (CUDA events
+                                        on the legacy stream; includes the host work between batches and the device-to-device copy
+                                        of the file set's data region) */
+} og_merge_info;
+OG_API int og_shard_merge_info(const og_shard *s, og_merge_info *out); /* og_shard_open / og_shard_synth shards: n_files = 1, zeros */
 
 /* ---- query (aggregate cursor tree) ---- */
 OG_API int og_query_create(og_shard *s, const og_query_desc *desc, og_query **out);

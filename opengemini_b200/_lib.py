@@ -23,6 +23,7 @@ Q_NO_FAST = 4
 Q_QUERY_GRID = 16
 SYNTH_F_HI, SYNTH_F_LO, SYNTH_INT_WALK, SYNTH_BOOL = 0, 1, 2, 3
 SHARD_DEVICE_DATA = 1
+FILE_OUT_OF_ORDER = 1
 
 u8p, u32p, u64p, i64p, i32p = C.POINTER(C.c_uint8), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(C.c_int64), C.POINTER(C.c_int32)
 
@@ -94,6 +95,13 @@ class ShardLayout(C.Structure):
     _fields_ = [("data_len", C.c_uint64), ("n_series", C.c_uint32), ("n_segments", C.c_uint32), ("n_columns", C.c_uint32)]
 
 
+class MergeInfo(C.Structure):
+    _fields_ = [("n_files", C.c_uint32), ("n_out_of_order_files", C.c_uint32), ("series_merged", C.c_uint64),
+                ("out_of_order_rows", C.c_uint64), ("rows_replaced", C.c_uint64), ("rows_after_merge", C.c_uint64),
+                ("segments_kept", C.c_uint64), ("segments_rewritten_in", C.c_uint64), ("segments_rewritten_out", C.c_uint64),
+                ("merge_ms", C.c_double)]
+
+
 # every symbol include/ogpu.h declares (checked by tests/test_abi.py against the header text)
 EXPORTS = [
     "og_init", "og_device_count", "og_strerror", "og_last_error", "og_version", "og_shard_open", "og_shard_close",
@@ -103,6 +111,7 @@ EXPORTS = [
     "og_release_cached_memory", "og_comm_unique_id", "og_comm_init_rank", "og_comm_destroy", "og_comm_info", "og_comm_allreduce_f64", "og_query_allreduce",
     "og_downsample", "og_downsampled_desc", "og_downsampled_export", "og_downsampled_free",
     "og_tssp_parse", "og_tssp_desc", "og_tssp_measurement", "og_tssp_time_range", "og_tssp_free",
+    "og_shard_open_files", "og_shard_merge_info",
 ]
 
 _lib = None
@@ -130,6 +139,8 @@ def lib():
     L.og_version.restype = C.c_char_p
     L.og_init.argtypes = [C.c_int]
     L.og_shard_open.argtypes = [C.POINTER(ShardDesc), C.POINTER(C.c_void_p)]
+    L.og_shard_open_files.argtypes = [C.POINTER(ShardDesc), u32p, C.c_uint32, C.POINTER(C.c_void_p)]
+    L.og_shard_merge_info.argtypes = [C.c_void_p, C.POINTER(MergeInfo)]
     L.og_shard_close.argtypes = [C.c_void_p]
     L.og_shard_close.restype = None
     L.og_shard_info.argtypes = [C.c_void_p, u64p, u64p, u64p, u64p, i64p, i64p]

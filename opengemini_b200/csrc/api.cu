@@ -202,44 +202,57 @@ OG_API void og_shard_close(og_shard *s) {
     delete s;
 }
 
+} // extern "C"
+namespace ogpu {
+/* host checks of one shard description: og_shard_open and og_shard_open_files (merge.cu) run them on every description */
+int check_desc(const og_shard_desc *d) {
+    if (d->n_columns > 64 || (d->n_segments && (!d->seg_tmin || !d->seg_tmax || !d->time_page_off || !d->time_page_len)) || (d->n_series && !d->series_seg_begin)) { set_error("bad shard descriptor"); return OG_E_INVAL; }
+    for (uint32_t s = 0; s < d->n_series; s++) if (d->series_seg_begin[s] > d->series_seg_begin[s + 1]) { set_error("series_seg_begin not monotone at %u", s); return OG_E_INVAL; }
+    if (d->n_series && d->series_seg_begin[d->n_series] != d->n_segments) { set_error("series_seg_begin[n_series] != n_segments"); return OG_E_INVAL; }
+    for (uint32_t c = 0; c < d->n_columns; c++)
+        if (d->columns[c].type != OG_TYPE_INT && d->columns[c].type != OG_TYPE_FLOAT && d->columns[c].type != OG_TYPE_BOOL && d->columns[c].type != OG_TYPE_STRING) {
+            set_error("column %u: unknown column type %d", c, d->columns[c].type); return OG_E_UNSUPPORTED;
+        }
+    for (size_t c = 0; c <= d->n_columns; c++) {
+        const uint64_t *po = c < d->n_columns ? d->columns[c].page_off : d->time_page_off;
+        const uint32_t *pl = c < d->n_columns ? d->columns[c].page_len : d->time_page_len;
+        for (size_t g = 0; g < d->n_segments; g++)
+            if (po[g] + pl[g] > d->data_len) { set_error("column %zu segment %zu: page [%llu,+%u) outside data (%llu bytes)", c, g, (unsigned long long)po[g], pl[g], (unsigned long long)d->data_len); return OG_E_INVAL; }
+    }
+    for (uint32_t sr = 0; sr < d->n_series; sr++)
+        for (uint32_t g = d->series_seg_begin[sr]; g < d->series_seg_begin[sr + 1]; g++)
+            if (d->seg_tmin[g] > d->seg_tmax[g] || (g > d->series_seg_begin[sr] && d->seg_tmin[g] <= d->seg_tmax[g - 1])) {
+                set_error("series %u: segment %u is not time-ordered (only ordered TSSP files are supported)", sr, g); return OG_E_UNSUPPORTED;
+            }
+    return OG_OK;
+}
+} // namespace ogpu
+extern "C" {
+
 OG_API int og_shard_open(const og_shard_desc *d, og_shard **out) {
     if (!d || !out) { set_error("null argument"); return OG_E_INVAL; }
     *out = nullptr;
     int rc = need_device(); if (rc) return rc;
-    if (d->n_columns > 64 || (d->n_segments && (!d->seg_tmin || !d->seg_tmax || !d->time_page_off || !d->time_page_len)) || (d->n_series && !d->series_seg_begin)) { set_error("bad shard descriptor"); return OG_E_INVAL; }
-    for (uint32_t s = 0; s < d->n_series; s++) if (d->series_seg_begin[s] > d->series_seg_begin[s + 1]) { set_error("series_seg_begin not monotone at %u", s); return OG_E_INVAL; }
-    if (d->n_series && d->series_seg_begin[d->n_series] != d->n_segments) { set_error("series_seg_begin[n_series] != n_segments"); return OG_E_INVAL; }
+    if ((rc = check_desc(d))) return rc;
     og_shard *s = new og_shard;
     s->device = g_device; s->n_series = d->n_series; s->n_segments = d->n_segments; s->n_columns = d->n_columns;
     s->data_len = d->data_len;
     for (uint32_t c = 0; c < d->n_columns; c++) {
         s->col_types.push_back(d->columns[c].type);
         s->col_names.push_back(d->columns[c].name ? d->columns[c].name : "");
-        if (d->columns[c].type != OG_TYPE_INT && d->columns[c].type != OG_TYPE_FLOAT && d->columns[c].type != OG_TYPE_BOOL && d->columns[c].type != OG_TYPE_STRING) {
-            set_error("column %u: unknown column type %d", c, d->columns[c].type); delete s; return OG_E_UNSUPPORTED;
-        }
     }
     s->sids.assign(d->sids, d->sids + d->n_series);
     s->h_series_seg_begin.assign(d->series_seg_begin, d->series_seg_begin + d->n_series + 1);
     size_t nseg = d->n_segments, ncol1 = (size_t)d->n_columns + 1;
-    /* bounds + ordering checks on the host directory */
     std::vector<uint64_t> off(ncol1 * nseg); std::vector<uint32_t> len(ncol1 * nseg);
     for (size_t c = 0; c < ncol1; c++) {
         const uint64_t *po = c < d->n_columns ? d->columns[c].page_off : d->time_page_off;
         const uint32_t *pl = c < d->n_columns ? d->columns[c].page_len : d->time_page_len;
-        for (size_t g = 0; g < nseg; g++) {
-            if (po[g] + pl[g] > d->data_len) { set_error("column %zu segment %zu: page [%llu,+%u) outside data (%llu bytes)", c, g, (unsigned long long)po[g], pl[g], (unsigned long long)d->data_len); delete s; return OG_E_INVAL; }
-            off[c * nseg + g] = po[g]; len[c * nseg + g] = pl[g];
-        }
+        for (size_t g = 0; g < nseg; g++) { off[c * nseg + g] = po[g]; len[c * nseg + g] = pl[g]; }
     }
     s->tmin = INT64_MAX; s->tmax = INT64_MIN;
-    for (uint32_t sr = 0; sr < d->n_series; sr++)
-        for (uint32_t g = d->series_seg_begin[sr]; g < d->series_seg_begin[sr + 1]; g++) {
-            if (d->seg_tmin[g] > d->seg_tmax[g] || (g > d->series_seg_begin[sr] && d->seg_tmin[g] <= d->seg_tmax[g - 1])) {
-                set_error("series %u: segment %u is not time-ordered (only ordered TSSP files are supported)", sr, g); delete s; return OG_E_UNSUPPORTED;
-            }
-            s->tmin = std::min(s->tmin, d->seg_tmin[g]); s->tmax = std::max(s->tmax, d->seg_tmax[g]);
-        }
+    if (d->n_series)
+        for (uint32_t g = d->series_seg_begin[0]; g < d->series_seg_begin[d->n_series]; g++) { s->tmin = std::min(s->tmin, d->seg_tmin[g]); s->tmax = std::max(s->tmax, d->seg_tmax[g]); }
 #define TRY(x) do { rc = (x); if (rc) { og_shard_close(s); return rc; } } while (0)
 #define TRYCU(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { rc = cuda_fail(e_, #x, __FILE__, __LINE__); og_shard_close(s); return rc; } } while (0)
     if (d->flags & OG_SHARD_DEVICE_DATA) { s->d_data = (uint8_t *)d->data; s->owns_data = false; }

@@ -123,7 +123,9 @@ __device__ bool gorilla_encode_dev(BitWriter &w, const SegIn &s, uint32_t limit_
     return true;
 }
 
-__device__ uint32_t encode_float_page(uint8_t *out, const SegIn &s, int *flags) {
+/* nan_raw: a segment that FloatArrayEncodeAll refuses (sum over src[1:] is NaN: +Inf and -Inf in one segment) gets the raw
+ * block instead of flag 2 (the open-time merge re-encodes rows it must not drop, merge.cu) */
+__device__ uint32_t encode_float_page(uint8_t *out, const SegIn &s, int *flags, bool nan_raw) {
     BitWriter w; w.init(out);
     if (s.rows == 1 && s.valid(0)) { w.put(17, 8); w.put_bytes_le64(s.cell(0)); return w.finish(); } /* CanEncodeOneRowMode :488 */
     uint32_t n = write_header(w, s, OG_TYPE_FLOAT);
@@ -189,7 +191,10 @@ __device__ uint32_t encode_float_page(uint8_t *out, const SegIn &s, int *flags) 
         if (flags) atomicOr(flags, 1);
         raw(); return w.finish();
     }
-    if (sum_tail != sum_tail && flags) atomicOr(flags, 2); /* "unsupported value: NaN" (+Inf and -Inf in one segment) */
+    if (sum_tail != sum_tail) { /* "unsupported value: NaN" (+Inf and -Inf in one segment) */
+        if (nan_raw) { raw(); return w.finish(); }
+        if (flags) atomicOr(flags, 2);
+    }
     w.put(0x30, 8);
     uint32_t limit = n * 8 * 90 / 100;
     bool fits = gorilla_encode_dev(w, s, hdr_bits / 8 + limit + 16);
@@ -316,7 +321,8 @@ __device__ uint32_t encode_bool_page(uint8_t *out, const SegIn &s) {
 
 /* one thread per segment: encode into staging[seg * PAGE_STRIDE], record the length */
 __global__ void k_encode_pages(int type, int is_time, const uint8_t *cells, const uint8_t *okb, const uint32_t *rows_arr,
-                               uint32_t n_segments, uint32_t rps, uint8_t *staging, uint32_t *lens, uint64_t *dense_scratch, int *flags) {
+                               uint32_t n_segments, uint32_t rps, uint8_t *staging, uint32_t *lens, uint64_t *dense_scratch, int *flags,
+                               bool nan_raw) {
     uint32_t seg = blockIdx.x * blockDim.x + threadIdx.x;
     if (seg >= n_segments) return;
     uint32_t rows = rows_arr ? rows_arr[seg] : rps;
@@ -327,7 +333,7 @@ __global__ void k_encode_pages(int type, int is_time, const uint8_t *cells, cons
     s.okb = okb ? okb + (size_t)seg * rps : nullptr;
     uint32_t len;
     if (is_time) len = encode_time_page(out, (const int64_t *)s.cells, rows, flags);
-    else if (type == OG_TYPE_FLOAT) len = encode_float_page(out, s, flags);
+    else if (type == OG_TYPE_FLOAT) len = encode_float_page(out, s, flags, nan_raw);
     else if (type == OG_TYPE_BOOL) len = encode_bool_page(out, s);
     else {
         if (s.okb) { /* compact the non-null ints so the delta logic sees ColVal.Val */
@@ -425,9 +431,11 @@ using namespace ogpu;
 
 extern "C" {
 
-OG_API int og_encode_pages(int32_t type, int32_t is_time, const void *d_values, const uint8_t *d_valid, const uint32_t *d_rows,
-                           uint32_t n_segments, uint32_t rps, uint8_t *d_out, uint64_t out_cap, uint64_t *d_page_off,
-                           uint32_t *d_page_len, uint64_t *total_bytes_out) {
+} // extern "C"
+namespace ogpu {
+/* og_encode_pages; nan_raw: see encode_float_page */
+int encode_pages(int32_t type, int32_t is_time, const void *d_values, const uint8_t *d_valid, const uint32_t *d_rows, uint32_t n_segments,
+                 uint32_t rps, uint8_t *d_out, uint64_t out_cap, uint64_t *d_page_off, uint32_t *d_page_len, uint64_t *total_bytes_out, bool nan_raw) {
     if (!d_values || !d_out || !d_page_off || !d_page_len || rps == 0 || rps > 1000) { set_error("bad argument (rows_per_segment must be 1..1000)"); return OG_E_INVAL; }
     if (type != OG_TYPE_INT && type != OG_TYPE_FLOAT && type != OG_TYPE_BOOL) { set_error("unsupported column type %d", type); return OG_E_UNSUPPORTED; }
     if (n_segments == 0) { if (total_bytes_out) *total_bytes_out = 0; return OG_OK; }
@@ -438,7 +446,7 @@ OG_API int og_encode_pages(int32_t type, int32_t is_time, const void *d_values, 
     if (type == OG_TYPE_INT && d_valid && !is_time && (rc = dalloc2(&dense, (size_t)n_segments * rps))) { dev_free(staging); return rc; }
     if ((rc = dalloc2(&flags, 1)) || (rc = dalloc2(&d_total, 1))) { dev_free(staging); dev_free(dense); return rc; }
     cudaMemset(flags, 0, 4);
-    k_encode_pages<<<(n_segments + 63) / 64, 64>>>(type, is_time, (const uint8_t *)d_values, is_time ? nullptr : d_valid, d_rows, n_segments, rps, staging, d_page_len, dense, flags);
+    k_encode_pages<<<(n_segments + 63) / 64, 64>>>(type, is_time, (const uint8_t *)d_values, is_time ? nullptr : d_valid, d_rows, n_segments, rps, staging, d_page_len, dense, flags, nan_raw);
     k_scan_lens<<<1, 1024>>>(d_page_len, n_segments, 0, d_page_off, d_total);
     k_compact_pages<<<(unsigned)(((size_t)n_segments * 32 + 255) / 256), 256>>>(staging, d_page_len, d_page_off, n_segments, d_out, out_cap, flags);
     unsigned long long total = 0; int fl = 0;
@@ -450,6 +458,14 @@ OG_API int og_encode_pages(int32_t type, int32_t is_time, const void *d_values, 
     if (fl & 16) { set_error("output buffer too small (%llu bytes needed)", total); return OG_E_NOMEM; }
     if (total_bytes_out) *total_bytes_out = total;
     return OG_OK;
+}
+} // namespace ogpu
+extern "C" {
+
+OG_API int og_encode_pages(int32_t type, int32_t is_time, const void *d_values, const uint8_t *d_valid, const uint32_t *d_rows,
+                           uint32_t n_segments, uint32_t rps, uint8_t *d_out, uint64_t out_cap, uint64_t *d_page_off,
+                           uint32_t *d_page_len, uint64_t *total_bytes_out) {
+    return encode_pages(type, is_time, d_values, d_valid, d_rows, n_segments, rps, d_out, out_cap, d_page_off, d_page_len, total_bytes_out, false);
 }
 
 OG_API int og_shard_synth(const og_synth_desc *dd, og_shard **out) {
@@ -495,12 +511,12 @@ OG_API int og_shard_synth(const og_synth_desc *dd, og_shard **out) {
         unsigned g = (n + 127) / 128;
         if (c == d.n_columns) {
             k_synth_times<<<g, 128>>>(d, b0, n, sps, (int64_t *)cells, rows_arr, s->d_tmin, s->d_tmax);
-            k_encode_pages<<<(n + 63) / 64, 64>>>(OG_TYPE_INT, 1, cells, nullptr, rows_arr, n, rps, staging, lens, nullptr, flags);
+            k_encode_pages<<<(n + 63) / 64, 64>>>(OG_TYPE_INT, 1, cells, nullptr, rows_arr, n, rps, staging, lens, nullptr, flags, false);
         } else {
             const og_synth_column &col = d.columns[c];
             k_synth_times<<<g, 128>>>(d, b0, n, sps, (int64_t *)cells, rows_arr, s->d_tmin, s->d_tmax); /* rows_arr (overwritten cells are refilled below) */
             k_synth_fill<<<g, 128>>>(d, col, c, b0, n, sps, cells, col.null_permille ? okb : nullptr);
-            k_encode_pages<<<(n + 63) / 64, 64>>>(col.type, 0, cells, col.null_permille ? okb : nullptr, rows_arr, n, rps, staging, lens, dense, flags);
+            k_encode_pages<<<(n + 63) / 64, 64>>>(col.type, 0, cells, col.null_permille ? okb : nullptr, rows_arr, n, rps, staging, lens, dense, flags, false);
         }
         k_scan_lens<<<1, 1024>>>(lens, n, base, offs, d_total);
         if (blob) {

@@ -45,6 +45,7 @@ struct og_shard {
     uint64_t irregular_time_pages = 0; /* time pages that are neither const-delta nor one-row (Simple8b / raw times) */
     uint64_t n_rows = 0, page_bytes = 0;
     uint64_t snappy_pages = 0, snappy_bytes_in = 0, snappy_bytes_out = 0; /* Snappy pages transcoded to raw at open */
+    og_merge_info merge{1, 0, 0, 0, 0, 0, 0, 0, 0, 0}; /* og_shard_open_files (merge.cu); one file and zeros otherwise */
     int64_t tmin = 0, tmax = 0;
     std::vector<uint64_t> sids;
     std::vector<int32_t> col_types;

@@ -4,6 +4,7 @@ The call sequence mirrors how the reference drives this path (engine/iterators.g
 aggregateCursor.SinkPlan -> KeyCursor.Next, engine/comm/cursor.go:46-56):
 
     shard = Shard.open(...) | Shard.synth(...)       # TSSP pages + flattened ChunkMeta resident in HBM
+          | Shard.open_files([(file, out_of_order), ...])  # a shard's file set, merged on the device at open
     q = AggQuery(shard, calls=[("sum", 0), ("count", 0)], interval=60e9, tmin=.., tmax=..)
     q.run()                                          # kernels
     for rec in q.records(): ...                      # Next(): ColVal-shaped views, (nil,nil,nil) == StopIteration
@@ -46,9 +47,10 @@ class Shard:
     def init(device=0):
         L.check(L.lib().og_init(device), "og_init")
 
-    @classmethod
-    def open(cls, data, sids, series_seg_begin, seg_tmin, seg_tmax, columns, time_page_off, time_page_len):
-        """columns: list of (name, type, page_off[u64], page_len[u32]); data: bytes/np.uint8 (host)."""
+    @staticmethod
+    def desc(data, sids, series_seg_begin, seg_tmin, seg_tmax, columns, time_page_off, time_page_len):
+        """An L.ShardDesc over host arrays (what Shard.open takes); the arrays it points at are kept alive as desc._keep.
+        columns: list of (name, type, page_off[u64], page_len[u32]); data: bytes/np.uint8 (host)."""
         data = np.ascontiguousarray(np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else data)
         sids = np.ascontiguousarray(sids, dtype=np.uint64)
         ssb = np.ascontiguousarray(series_seg_begin, dtype=np.uint32)
@@ -80,9 +82,47 @@ class Shard:
         d.time_page_off = _ptr(tpo, C.c_uint64)
         d.time_page_len = _ptr(tpl, C.c_uint32)
         d.flags = 0
+        d._keep = (keep, cds)
+        return d
+
+    @classmethod
+    def open(cls, data, sids, series_seg_begin, seg_tmin, seg_tmax, columns, time_page_off, time_page_len):
+        """columns: list of (name, type, page_off[u64], page_len[u32]); data: bytes/np.uint8 (host)."""
+        d = cls.desc(data, sids, series_seg_begin, seg_tmin, seg_tmax, columns, time_page_off, time_page_len)
         h = C.c_void_p()
         L.check(L.lib().og_shard_open(C.byref(d), C.byref(h)), "og_shard_open")
         return cls(h.value)
+
+    @classmethod
+    def open_files(cls, files):
+        """One shard from its ordered and out-of-order files (og_shard_open_files): files = [(desc_or_tssp_bytes, out_of_order)]
+        in file-sequence order, oldest first.  A file is an L.ShardDesc (Shard.desc) or a TSSP file image, which goes through
+        og_tssp_parse / og_tssp_desc.  Overlapping rows are merged on the device as the shard opens; merge_info() reports it."""
+        descs = (L.ShardDesc * len(files))()
+        flags = np.array([L.FILE_OUT_OF_ORDER if ooo else 0 for _f, ooo in files], dtype=np.uint32)
+        keep, parsed = [], []
+        try:
+            for i, (f, _ooo) in enumerate(files):
+                if isinstance(f, L.ShardDesc):
+                    C.memmove(C.byref(descs[i]), C.byref(f), C.sizeof(L.ShardDesc))
+                    continue
+                buf = np.frombuffer(f, dtype=np.uint8) if not isinstance(f, np.ndarray) else np.ascontiguousarray(f, dtype=np.uint8)
+                keep.append(buf)
+                t = C.c_void_p()
+                L.check(L.lib().og_tssp_parse(buf.ctypes.data, buf.size, C.byref(t)), "og_tssp_parse")
+                parsed.append(t)
+                L.check(L.lib().og_tssp_desc(t, C.byref(descs[i])), "og_tssp_desc")
+            h = C.c_void_p()
+            L.check(L.lib().og_shard_open_files(descs, _ptr(flags, C.c_uint32), len(files), C.byref(h)), "og_shard_open_files")
+        finally:
+            for t in parsed:
+                L.lib().og_tssp_free(t)
+        return cls(h.value)
+
+    def merge_info(self):
+        m = L.MergeInfo()
+        L.check(L.lib().og_shard_merge_info(self.h, C.byref(m)), "og_shard_merge_info")
+        return {k: getattr(m, k) for k, _ in L.MergeInfo._fields_}
 
     @classmethod
     def open_desc(cls, desc, keepalive=None):
