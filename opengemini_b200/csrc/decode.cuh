@@ -5,9 +5,10 @@
  * the (valid, value) of the next row of one field column, straight from the page bytes.  Every generic consumer — shard
  * validation, the materialise kernels, the decode step of the tile path and the pull-iterator aggregate kernel — uses these
  * two iterators, so they all agree on what a corrupt page is.  A consumer that walks a page to its last row calls finish(),
- * which checks that the words / runs hold exactly the page's value count.  The one exception is k_fused_cols (fused_cols.cuh):
- * it decodes Gorilla, Simple8b and bool pages in loops of its own, pulls the other codecs through ColIter::value(), and does
- * not run the end-of-page checks.  Shard open (k_validate) guarantees that a page's validity bits mark exactly
+ * which checks that the words / runs hold exactly the page's value count.  k_fused_cols (fused_cols.cuh) decodes Gorilla,
+ * Simple8b and bool pages in loops of its own and pulls the other codecs through ColIter::value(); a pass of it that reaches a
+ * segment's last row runs the same checks (finish() for the ColIter codecs, their restatement for its Simple8b loop).  Shard
+ * open (k_validate) guarantees that a page's validity bits mark exactly
  * rows - nil_count rows valid, so no iterator takes more values from a block than its header counts.  Formats follow
  * SURVEY.md App.A; reference functions replaced:
  *   parse_field_header   engine/immutable/column_builder.go:446-486 DecodeColumnHeader, reader.go:700 DecodeColumnOfOneValue

@@ -238,6 +238,12 @@ __device__ __forceinline__ void cols_pass(const QueryP &q, const ChunkP &ch, con
     if (MODE == 1 && (sg.r_hi & 31) != 31) keep[sg.r_hi >> 5] = kw;
     };
     if (!bm && all_ok) run(std::true_type{}); else run(std::false_type{});
+    /* a pass that walked to the segment's last row has taken every value of the block: the end-of-page checks of
+     * ColIter::finish (every Simple8b slot of every word taken, no word left, exactly n values; RLE runs add up to n) */
+    if (sg.r_hi + 1 == sg.rows) {
+        if (KIND == CK_GENERIC) it.finish();
+        else if (KIND == CK_S8B && (idx != it.h.rows - it.h.nil_count || sleft != 0 || swords != 0)) it.err = D_CORRUPT;
+    }
 }
 
 template <int MODE, bool SIMPLE>

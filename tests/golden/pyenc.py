@@ -99,6 +99,8 @@ def gorilla(values):
 def _is_int(f):
     if 0 <= f < (1 << 32):
         return float(int(f)) == f
+    if math.isinf(f):                                   # Go: math.Ceil(+-Inf) == +-Inf (Python's math.ceil raises)
+        return True
     return math.ceil(f) == f and math.floor(f) == f
 
 

@@ -282,7 +282,7 @@ def test_payload_that_disagrees_with_the_value_count(monkeypatch):
     gorilla_cut = gpage[:15 + (gpage.size - 15) // 2]  # half the bit stream
 
     def paths(typ, page):
-        """(label, run) for og_decode_segment, path 1, path 0 and path 4; run() returns the dense result of the aggregates"""
+        """(label, run) for og_decode_segment and paths 1, 0, 4 and 5; run() returns the dense result of the aggregates"""
         sh = _one_segment_shard(typ, page, tp, t, n_cols=2)
 
         def query(calls, flags, path):
@@ -301,7 +301,8 @@ def test_payload_that_disagrees_with_the_value_count(monkeypatch):
         return sh, [("decode", lambda: sh.decode_segment(0)),
                     ("path 1", lambda: query([("sum", 0), ("count", 0), ("max", 0)], L.Q_NO_FAST, 1)),
                     ("path 0", lambda: query([("sum", 0), ("count", 0), ("max", 0)], L.Q_NO_FUSED, 0)),
-                    ("path 4", multi)]
+                    ("path 4", multi),
+                    ("path 5", lambda: query([("sum", 0), ("count", 1), ("max", 0)], 0, 5))]
 
     for label, typ, page in (("s8b surplus word", L.TYPE_INT, surplus), ("s8b missing word", L.TYPE_INT, missing),
                              ("rle n+1", L.TYPE_FLOAT, rle_n1), ("rle zero-length value run", L.TYPE_FLOAT, rle_value0),
