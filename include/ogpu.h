@@ -222,6 +222,7 @@ typedef struct og_stats {
     uint64_t il_bytes;         /* its size in HBM */
     uint64_t general_segments; /* segments of the column that the Gorilla kernel does not take (other codecs, nulls, irregular time pages) */
     double merge_ms;           /* device time of the last og_query_allreduce (pack + collectives + fold) */
+    uint64_t il_packed_segments; /* segments of that copy stored as fixed-width XOR deltas rather than Gorilla records */
 } og_stats;
 
 typedef struct og_shard og_shard;

@@ -78,7 +78,8 @@ class Stats(C.Structure):
     _fields_ = [("rows_decoded", C.c_uint64), ("segments_scanned", C.c_uint64), ("page_bytes", C.c_uint64),
                 ("dir_bytes", C.c_uint64), ("out_bytes", C.c_uint64), ("kernel_ms", C.c_double), ("h2d_ms", C.c_double), ("main_kernel_ms", C.c_double),
                 ("kernel_launches", C.c_uint32), ("path", C.c_int32), ("il_state", C.c_int32), ("per_series_cells_used", C.c_int32),
-                ("il_build_ms", C.c_double), ("il_bytes", C.c_uint64), ("general_segments", C.c_uint64), ("merge_ms", C.c_double)]
+                ("il_build_ms", C.c_double), ("il_bytes", C.c_uint64), ("general_segments", C.c_uint64), ("merge_ms", C.c_double),
+                ("il_packed_segments", C.c_uint64)]
 
 
 class SynthColumn(C.Structure):

@@ -196,7 +196,7 @@ OG_API void og_shard_close(og_shard *s) {
     if (s->h_seg_buf) cudaFreeHost(s->h_seg_buf);
     if (s->d_seg_buf) dev_free(s->d_seg_buf);
     for (auto &c : s->il) {
-        dev_free(c.words); dev_free(c.grp_off); dev_free(c.grp_rows); dev_free(c.grp_col); dev_free(c.ok); dev_free(c.lane_seg); dev_free(c.lane_rows);
+        dev_free(c.words); dev_free(c.grp_off); dev_free(c.grp_rows); dev_free(c.grp_col); dev_free(c.lane_seg); dev_free(c.lane_rows); dev_free(c.lane_win);
         dev_free(c.lane_series); dev_free(c.lane_t0); dev_free(c.lane_dt); dev_free(c.gen_list);
     }
     delete s;
@@ -548,14 +548,14 @@ int ensure_il(og_shard *s, int col, cudaStream_t st) {
     TmpBufs tmp;
     IlScanOut so{};
     uint32_t *seg_words; uint64_t *keys2; uint32_t *vals2;
-    if ((rc = dalloc(&ic.ok, (size_t)nseg))) return rc;
-    so.ok = ic.ok;
-    if ((rc = tmp.get(&seg_words, nseg)) || (rc = tmp.get(&so.seg_t0, nseg)) || (rc = tmp.get(&so.seg_dt, nseg)) || (rc = tmp.get(&so.keys, nseg)) ||
+    if ((rc = tmp.get(&so.seg_win, nseg)) || (rc = tmp.get(&so.n_packed, 1)) ||
+        (rc = tmp.get(&seg_words, nseg)) || (rc = tmp.get(&so.seg_t0, nseg)) || (rc = tmp.get(&so.seg_dt, nseg)) || (rc = tmp.get(&so.keys, nseg)) ||
         (rc = tmp.get(&so.vals, nseg)) || (rc = tmp.get(&keys2, nseg)) || (rc = tmp.get(&vals2, nseg)) || (rc = tmp.get(&so.dom_cnt, n_dom))) return rc;
     so.seg_words = seg_words;
     if ((rc = tmp.get(&so.misaligned, 1))) return rc;
     CU(cudaMemsetAsync(so.dom_cnt, 0, (size_t)n_dom * 4, st));
     CU(cudaMemsetAsync(so.misaligned, 0, 4, st));
+    CU(cudaMemsetAsync(so.n_packed, 0, 8, st));
     DirP d = make_dir(s);
     k_il_scan<<<(nseg + 255) / 256, 256, 0, st>>>(d, col, s->col_types[col], J, so);
     CU(cudaGetLastError());
@@ -567,9 +567,10 @@ int ensure_il(og_shard *s, int col, cudaStream_t st) {
         void *dtmp; if ((rc = tmp.get((uint8_t **)&dtmp, tb))) return rc;
         CU(cub::DeviceRadixSort::SortPairs(dtmp, tb, so.keys, keys2, so.vals, vals2, (int)nseg, 0, (int)OG_IL_WORD_BITS + dbits, st));
     }
-    std::vector<uint32_t> dom_cnt(n_dom); uint32_t misaligned = 1;
+    std::vector<uint32_t> dom_cnt(n_dom); uint32_t misaligned = 1; unsigned long long n_packed = 0;
     CU(cudaMemcpyAsync(dom_cnt.data(), so.dom_cnt, (size_t)n_dom * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(&misaligned, so.misaligned, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&n_packed, so.n_packed, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     std::vector<uint32_t> elem_first(n_dom), grp_first(n_dom);
     uint64_t n_elig = 0, ng64 = 0;
@@ -593,15 +594,16 @@ int ensure_il(og_shard *s, int col, cudaStream_t st) {
     CU(cudaMemcpyAsync(d_elem_first, elem_first.data(), (size_t)n_dom * 4, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(d_grp_first, grp_first.data(), (size_t)n_dom * 4, cudaMemcpyHostToDevice, st));
     const size_t n_slots = (size_t)ng * 32;
-    if ((rc = dalloc(&ic.lane_seg, n_slots)) || (rc = dalloc(&ic.lane_rows, n_slots)) || (rc = dalloc(&ic.lane_series, n_slots)) ||
+    if ((rc = dalloc(&ic.lane_seg, n_slots)) || (rc = dalloc(&ic.lane_rows, n_slots)) || (rc = dalloc(&ic.lane_win, n_slots)) || (rc = dalloc(&ic.lane_series, n_slots)) ||
         (rc = dalloc(&ic.lane_t0, n_slots)) || (rc = dalloc(&ic.lane_dt, n_slots)) || (rc = dalloc(&ic.grp_col, (size_t)ng)) ||
         (rc = dalloc(&ic.grp_rows, (size_t)ng)) || (rc = dalloc(&ic.grp_off, (size_t)ng))) return rc;
     CU(cudaMemsetAsync(ic.lane_seg, 0xff, n_slots * 4, st));
     CU(cudaMemsetAsync(ic.lane_rows, 0, n_slots * 4, st));
+    CU(cudaMemsetAsync(ic.lane_win, 0, n_slots * 2, st));
     IlAssign as{};
     as.keys = keys2; as.segs = vals2; as.elem_first = d_elem_first; as.grp_first = d_grp_first;
-    as.seg_words = seg_words; as.seg_t0 = so.seg_t0; as.seg_dt = so.seg_dt; as.ok = ic.ok;
-    as.lane_seg = ic.lane_seg; as.lane_rows = ic.lane_rows; as.lane_series = ic.lane_series; as.grp_col = ic.grp_col; as.lane_t0 = ic.lane_t0; as.lane_dt = ic.lane_dt;
+    as.seg_words = seg_words; as.seg_t0 = so.seg_t0; as.seg_dt = so.seg_dt; as.seg_win = so.seg_win;
+    as.lane_seg = ic.lane_seg; as.lane_rows = ic.lane_rows; as.lane_series = ic.lane_series; as.grp_col = ic.grp_col; as.lane_win = ic.lane_win; as.lane_t0 = ic.lane_t0; as.lane_dt = ic.lane_dt;
     as.n_elig = (uint32_t)n_elig; as.J = J; as.cols_per_super = ic.cols_per_super;
     k_il_assign<<<(unsigned)((n_elig + 255) / 256), 256, 0, st>>>(d, as);
     k_il_group_rows<<<(unsigned)((n_slots + 255) / 256), 256, 0, st>>>(ng, ic.lane_seg, seg_words, ic.grp_rows);
@@ -620,12 +622,12 @@ int ensure_il(og_shard *s, int col, cudaStream_t st) {
         return OG_OK;
     }
     CU(cudaMemcpyAsync(ic.grp_off, go.data(), (size_t)ng * 8, cudaMemcpyHostToDevice, st));
-    k_il_repack<<<(unsigned)((n_slots + 127) / 128), 128, 0, st>>>(d, col, ic.ok, ic.lane_seg, ic.grp_off, ic.grp_rows, ng, ic.words);
+    k_il_repack<<<(unsigned)((n_slots + 127) / 128), 128, 0, st>>>(d, col, ic.lane_seg, ic.lane_win, ic.grp_off, ic.grp_rows, ng, ic.words);
     CU(cudaGetLastError());
     cudaEventRecord(ev1.e, st);
     CU(cudaStreamSynchronize(st));
     float ms = 0; cudaEventElapsedTime(&ms, ev0.e, ev1.e);
-    ic.n_words = total; ic.build_ms = ms; ic.state = 1;
+    ic.n_words = total; ic.n_packed = n_packed; ic.build_ms = ms; ic.state = 1;
     return OG_OK;
 }
 
@@ -755,7 +757,7 @@ int build_plan(og_query *q) {
     }
     if (pl->fast) {
         pl->il.words = ic->words; pl->il.grp_off = ic->grp_off; pl->il.grp_rows = ic->grp_rows; pl->il.grp_col = ic->grp_col;
-        pl->il.lane_seg = ic->lane_seg; pl->il.lane_rows = ic->lane_rows; pl->il.lane_series = ic->lane_series; pl->il.lane_t0 = ic->lane_t0; pl->il.lane_dt = ic->lane_dt;
+        pl->il.lane_seg = ic->lane_seg; pl->il.lane_rows = ic->lane_rows; pl->il.lane_win = ic->lane_win; pl->il.lane_series = ic->lane_series; pl->il.lane_t0 = ic->lane_t0; pl->il.lane_dt = ic->lane_dt;
         pl->fm = 0; pl->times = false;
         for (uint32_t c = 0; c < p.n_calls; c++) {
             pl->fm |= 1 << (p.calls[c].func - 1);
@@ -918,7 +920,7 @@ OG_API int og_query_run(og_query *q) {
     for (uint32_t c = 0; c < p.n_calls; c++) stt.out_bytes += cells_dense * (9 + (q->dense[c].tim ? 8 : 0));
     if (p.n_cols == 1 && p.col_type[0] == OG_TYPE_FLOAT && p.col_index[0] < (int)s->il.size()) {
         const og_shard::IlCol &ic = s->il[p.col_index[0]];
-        stt.il_state = ic.state; stt.il_build_ms = ic.build_ms; stt.il_bytes = ic.n_words * 4;
+        stt.il_state = ic.state; stt.il_build_ms = ic.build_ms; stt.il_bytes = ic.n_words * 4; stt.il_packed_segments = ic.state == 1 ? ic.n_packed : 0;
         stt.general_segments = ic.state == 1 ? (uint64_t)ic.gen_host.size() : s->n_segments;
     }
     stt.per_series_cells_used = err[2] != 0;

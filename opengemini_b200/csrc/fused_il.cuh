@@ -21,8 +21,12 @@
  *   decode    stateless bit addressing: three LDS.32 at immediate row offsets + two funnel shifts give the 64 stream bits
  *             at bit position q.  q is kept so that the '10' (window reuse) record's payload lands in place:
  *             q = p + 2 - leading  =>  val ^= x & MASK, and the two control bits are tested inside x with one LOP3.
- *             Raw pages are transcoded by the repack into fixed 64-bit XOR deltas, which the same path decodes with
- *             MASK = ~0 and no control bits — there is no separate raw-page kernel.
+ *   packed    a lane may instead hold its segment as fixed-width XOR deltas (il_build.cuh): the first value in 64 bits, then
+ *             (v_i ^ v_i-1) >> trail in m bits each, where [lead, lead + m) is the OR of all the segment's deltas.  The same
+ *             path decodes it with q = p - lead, MASK = the window, kfast = m and no control bits (CM = CE = 0): every
+ *             record lands in place and the lane never takes slow_record.  Raw pages are always stored so (there is no
+ *             separate raw-page kernel), and Gorilla pages whenever that is fewer words — high-entropy data such as G-hi,
+ *             whose deltas all sit in one 46-bit window, costs 46 bits a row instead of Gorilla's ~48.6.
  *   reduce    window boundaries are row countdowns derived from the const-delta time page; rounds in which no lane reaches
  *             a boundary run without the per-record test.  Partials stay in registers.  When the query has one tagset and
  *             the lanes share a time grid, the 32 partials of a bucket are folded with warp shuffles and ONE cell per
@@ -67,7 +71,7 @@ __device__ __forceinline__ bool mbar_wait(uint32_t bar, uint32_t parity) {
 }
 
 enum { FM_COUNT = 1, FM_SUM = 2, FM_MIN = 4, FM_MAX = 8, FM_FIRST = 16, FM_LAST = 32 };
-enum { SEG_GENERAL = 0, SEG_FAST = 1, SEG_RAWX = 2 }; /* static per-segment classes (k_il_scan): general kernel / Gorilla stream / raw page transcoded to XOR deltas */
+enum { SEG_GENERAL = 0, SEG_FAST = 1, SEG_PACKED = 2 }; /* static per-segment classes (k_il_scan): general kernel / Gorilla stream / fixed-width XOR deltas */
 
 #ifndef OG_FAST_THREADS
 #define OG_FAST_THREADS 128
@@ -94,10 +98,13 @@ enum { SEG_GENERAL = 0, SEG_FAST = 1, SEG_RAWX = 2 }; /* static per-segment clas
 #define OG_IL_HDR 7u            /* page = [31][rows u32][0x30][0x10] | stream: first value 8 B BE, records... */
 #define OG_IL_RAW_HDR 6u        /* page = [31][rows u32][0x00] | rows x 8 B LE */
 #define OG_IL_NONE 0xffffffffu
-#define OG_IL_RAWFLAG 0x80000000u
+/* lane_win of a packed lane: OG_IL_PACKED | lead << 8 | m (lead <= 63, m <= 64); 0 = Gorilla stream */
+#define OG_IL_PACKED 0x8000u
 /* bits past q that the next K records may touch: K records of <= 77 bits, q = p - sr with sr <= 29, the '11' header (13),
- * one 64-bit fetch and the word rounding of the three-row read */
+ * one 64-bit fetch and the word rounding of the three-row read.  A packed lane stays inside it for K >= 2: q = p - lead with
+ * lead <= 63 and K fields of <= 64 bits, so K*64 + 63 + 64 + 64 bits past q */
 #define OG_IL_LOOKBITS (77u * OG_IL_K + 29u + 13u + 64u + 64u)
+static_assert(OG_IL_K >= 2, "packed lanes: K*64 + 63 + 128 <= OG_IL_LOOKBITS needs K >= 2");
 static_assert(OG_IL_NW % OG_IL_B == 0 && (OG_IL_NW & (OG_IL_NW - 1)) == 0, "ring geometry");
 static_assert(OG_IL_NW - OG_IL_B > (OG_IL_LOOKBITS + 31u) / 32u + 2u, "ring too small for the round length: the slowest lane could not proceed");
 
@@ -108,7 +115,8 @@ struct IlP {
     const uint32_t *grp_rows;    /* [n_groups] rows of the group (multiple of OG_IL_B), 0 = no lane */
     const uint32_t *grp_col;     /* [n_groups] column of the group in the folded cell matrix (rank inside its segment index) */
     const uint32_t *lane_seg;    /* [n_groups*32] segment of every lane slot, OG_IL_NONE = empty */
-    const uint32_t *lane_rows;   /* rows of the segment | OG_IL_RAWFLAG for transcoded raw pages */
+    const uint32_t *lane_rows;   /* rows of the segment */
+    const uint16_t *lane_win;    /* OG_IL_PACKED | lead << 8 | m for a packed lane, 0 for a Gorilla stream */
     const uint32_t *lane_series; /* series index of the segment */
     const int64_t *lane_t0;      /* const-delta time page: t(r) = t0 + r*dt */
     const uint64_t *lane_dt;
@@ -193,12 +201,11 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
     if (!__any_sync(FULL, active)) return;
     const size_t e = 2 * (size_t)(seg - ch.seg_begin);
 
-    uint32_t rows = 0, series = 0, r_lo = 0, r_hi = 0; bool rawx = false;
+    uint32_t rows = 0, series = 0, r_lo = 0, r_hi = 0, lwin = 0;
     int64_t t0 = 0, dt = 1; uint64_t dtu = 1; double inv_dt = 1.0;
     const double inv_iv = 1.0 / __ull2double_rn((uint64_t)q.interval);
     if (active) {
-        const uint32_t rf = il.lane_rows[slot];
-        rows = rf & ~OG_IL_RAWFLAG; rawx = (rf & OG_IL_RAWFLAG) != 0; series = il.lane_series[slot];
+        rows = il.lane_rows[slot]; lwin = il.lane_win[slot]; series = il.lane_series[slot];
         t0 = il.lane_t0[slot]; dtu = il.lane_dt[slot]; dt = (int64_t)dtu;
         inv_dt = 1.0 / __ull2double_rn(dtu);
         /* rows inside [tmin, tmax] (FilterByTime) */
@@ -385,8 +392,11 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
 #endif
     if (active && !hung) {
         val = fetch64(col, 0); qp = 64; /* first value: 64 raw bits */
-        if (rawx) { MASK = ~0ull; kfast = 64; } /* transcoded raw page: a 64-bit XOR delta per row, no control bits */
-        else { CM = 0; CE = 1; } /* no window yet: the first record takes the general path */
+        if (lwin & OG_IL_PACKED) { /* m-bit deltas of the window [lead, lead + m): in place at q = p - lead, no control bits */
+            const uint32_t lead = (lwin >> 8) & 63u, mw = lwin & 127u;
+            qp = 64 - lead; kfast = mw;
+            MASK = mw ? (~0ull >> (64 - mw)) << (64 - lead - mw) : 0ull; /* m = 0: a constant segment, the lane never moves */
+        } else { CM = 0; CE = 1; } /* Gorilla, no window yet: the first record takes the general path */
     }
 
     /* ---- row events: skip rows before r_lo, window boundaries, end at r_hi ---- */

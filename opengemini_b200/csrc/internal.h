@@ -65,13 +65,13 @@ struct og_shard {
     std::vector<og_colval_view> seg_views;
     /* lane-interleaved, length-binned stream copy per column for the fused Gorilla kernel (fused_il.cuh), built on first use */
     struct IlCol { int state = 0; /* 0 not built, 1 ready, -1 no eligible segment, -2 not enough device memory (general kernel serves the column) */
-                   uint32_t *words = nullptr; uint64_t *grp_off = nullptr; uint32_t *grp_rows = nullptr, *grp_col = nullptr; uint8_t *ok = nullptr;
-                   uint32_t *lane_seg = nullptr, *lane_rows = nullptr, *lane_series = nullptr; int64_t *lane_t0 = nullptr; uint64_t *lane_dt = nullptr;
+                   uint32_t *words = nullptr; uint64_t *grp_off = nullptr; uint32_t *grp_rows = nullptr, *grp_col = nullptr;
+                   uint32_t *lane_seg = nullptr, *lane_rows = nullptr, *lane_series = nullptr; uint16_t *lane_win = nullptr; int64_t *lane_t0 = nullptr; uint64_t *lane_dt = nullptr;
                    uint32_t *gen_list = nullptr; std::vector<uint32_t> gen_host; /* segments the fused kernel does not take (ascending), device + host */
                    uint32_t n_groups = 0, J = 0; /* J != 0: regular shard, lane groups share a segment index */
                    bool aligned = false; /* regular shard whose segment index j has one [seg_tmin, seg_tmax] in every series of a binning domain */
                    uint32_t n_super = 1, cols_per_super = 0; std::vector<uint32_t> super_grp_first; /* [n_super+1] first lane group of each block of OG_IL_SUPER series */
-                   uint64_t n_words = 0; double build_ms = 0; };
+                   uint64_t n_words = 0, n_packed = 0; /* words of the copy; segments stored as packed XOR deltas */ double build_ms = 0; };
     std::vector<IlCol> il; /* [n_columns] */
     std::mutex il_mu;      /* queries of one shard may be planned from different threads: the build is serialised */
 };
