@@ -292,6 +292,8 @@ typedef struct og_merge_info {
 OG_API int og_shard_merge_info(const og_shard *s, og_merge_info *out); /* og_shard_open / og_shard_synth shards: n_files = 1, zeros */
 
 /* ---- query (aggregate cursor tree) ---- */
+/* OG_E_UNSUPPORTED when the first or last row in range lies in a window that Window() clamps at the int64 time limits
+ * (DESIGN.md "Deviations") */
 OG_API int og_query_create(og_shard *s, const og_query_desc *desc, og_query **out);
 OG_API int og_query_run(og_query *q);              /* launches the decode+aggregate kernels and waits for them */
 OG_API int og_query_next(og_query *q, og_record_view *out); /* OG_OK + record, or OG_EOF */

@@ -324,6 +324,17 @@ static void window_of(int64_t interval, int64_t offset, int64_t tmin, int64_t tm
     en += offset;
     *s = st; *e = en;
 }
+/* Window() clamps the window of t at MIN_TIME or MAX_TIME when the aligned window would reach past them.  The kernels place
+ * row t in bucket (t - start) / interval, which holds only on the unclamped grid, so og_query_create refuses a range whose
+ * first or last row lies in a clamped window (DESIGN.md "Deviations").  The window after the last row may be clamped: it
+ * only sets the bucket count, and every row still has its bucket. */
+static bool window_clamped(int64_t interval, int64_t offset, int64_t t) {
+    const __int128 x = (__int128)t - offset;
+    __int128 r = x % interval;
+    if (r < 0) r += interval;
+    const __int128 s = x - r, e = s + interval;
+    return s < MIN_TIME || e > MAX_TIME || s + offset < INT64_MIN || e + offset > INT64_MAX;
+}
 
 } /* extern "C" */
 namespace { void free_plan(void *plan); }
@@ -407,14 +418,19 @@ OG_API int og_query_create(og_shard *s, const og_query_desc *d_in, og_query **ou
     /* FileInfo.{Min,Max}Time is the file range intersected with the query range (fileLoopCursor.updateQueryTime :448-463),
      * so open-ended queries (opt.StartTime/EndTime = Min/MaxTime) get a bounded interval record. */
     int64_t gmin = std::max(d->tmin, s->tmin), gmax = std::min(d->tmax, s->tmax);
-    if (gmin > gmax) gmin = gmax = d->tmin; /* no overlap: one empty window */
+    bool overlap = gmin <= gmax;
+    if (!overlap) gmin = gmax = d->tmin; /* no overlap: one empty window */
     if (d->flags & OG_Q_QUERY_GRID) { /* one grid for every shard of a cross-shard query */
         if (d_in->tmin <= MIN_TIME || d_in->tmax >= MAX_TIME) { set_error("OG_Q_QUERY_GRID needs a bounded time range"); delete q; return OG_E_INVAL; }
-        gmin = d->tmin; gmax = d->tmax;
+        gmin = d->tmin; gmax = d->tmax; overlap = true;
     }
     int64_t s0, e0, s1, e1;
     if (d->interval == 0) { s0 = gmin; e0 = gmax + 1; s1 = s0; e1 = e0; }
     else {
+        /* (a range without rows keeps its one empty window, clamped or not: nothing is placed in it) */
+        if (overlap && (window_clamped(d->interval, d->offset, gmin) || window_clamped(d->interval, d->offset, gmax))) {
+            set_error("the first or last window of the range is clamped at the int64 time limits"); delete q; return OG_E_UNSUPPORTED;
+        }
         window_of(d->interval, d->offset, d->tmin, d->tmax, gmin, &s0, &e0);
         window_of(d->interval, d->offset, d->tmin, d->tmax, gmax + 1, &s1, &e1);
     }

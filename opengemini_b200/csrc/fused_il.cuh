@@ -212,7 +212,13 @@ __global__ void __maxnreg__(OG_FAST_MAXREG) k_fused_il(QueryP q, ChunkP ch, IlP 
         r_lo = 0; r_hi = rows - 1;
         if (t0 < q.tmin) { uint64_t k = udiv_est((uint64_t)(q.tmin - t0) + dtu - 1, dtu, inv_dt); r_lo = k > rows ? rows : (uint32_t)k; }
         { int64_t t_last = t0 + (int64_t)(rows - 1) * dt; if (t_last > q.tmax) { if (q.tmax < t0) r_lo = rows; else r_hi = (uint32_t)udiv_est((uint64_t)(q.tmax - t0), dtu, inv_dt); } }
-        if (r_lo > r_hi || r_lo >= rows) { *(uint2 *)(ch.edge_bucket + e) = make_uint2(OG_NO_BUCKET, OG_NO_BUCKET); active = false; }
+        /* rows in range outside the buckets [0, n_buckets): cannot happen on a validated shard, and must never become a stray
+         * cell store (the lane leaves as if it had no rows) */
+        const uint64_t span = (uint64_t)q.n_buckets * (uint64_t)q.interval;
+        const bool outside = r_lo <= r_hi && r_lo < rows &&
+                             ((uint64_t)(t0 + (int64_t)r_lo * dt - q.start) >= span || (uint64_t)(t0 + (int64_t)r_hi * dt - q.start) >= span);
+        if (outside) report_err(ch.err, D_CORRUPT, seg);
+        if (r_lo > r_hi || r_lo >= rows || outside) { *(uint2 *)(ch.edge_bucket + e) = make_uint2(OG_NO_BUCKET, OG_NO_BUCKET); active = false; }
     }
     if (!__any_sync(FULL, active)) return;
 
