@@ -50,7 +50,8 @@ struct ChunkP { /* one chunk of whole series */
     uint32_t J;                        /* segments per series on a regular shard, else 0 */
     int *err;                          /* [0] first error code, [1] segment */
     int *flags;                        /* [0] != 0: some kernel wrote per-series cells in this run (the cell merges have work);
-                                          [1] != 0: k_fused_il or k_fused_segment wrote edge windows (k_fix_edges_fold has work) */
+                                          [1] != 0: k_fused_il, k_fused_segment or k_fused_multi wrote edge windows
+                                          (k_fix_edges_fold has work) */
 };
 
 __device__ __forceinline__ size_t cell_idx(const ChunkP &ch, uint32_t series, uint32_t b) { return (size_t)(series - ch.series_begin) * ch.nb + b; }
@@ -71,6 +72,53 @@ __device__ __forceinline__ void store_cell(const ChunkP &ch, int call, uint32_t 
     store_part(ch.cells[call], cell_idx(ch, series, b), p);
     ch.flags[0] = 1;
 }
+
+/* Where one segment's window partials go, for the kernels that walk a segment's rows in time order in one thread (k_fused_multi,
+ * k_fused_segment): the first window with in-range rows (head) to edges[e], the last one (tail) to edges[e + 1], the windows
+ * between to the per-series cells; edge_bucket names the head and tail buckets for k_fix_edges.  The caller accumulates the rows
+ * of the open window into `parts` left to right, which keeps float sums in the reference's order (series_agg_func.gen.go:48-60).
+ * The kernels keep their prologue (pruning, time page, edge_bucket of a segment without rows) inline: as a member of this struct
+ * it changed the register allocation of several k_fused_multi instances. */
+struct SegWindows {
+    const QueryP &q; const ChunkP &ch;
+    const uint32_t seg; const size_t e; const uint32_t series;
+    uint32_t cur_b = OG_NO_BUCKET, head_b = OG_NO_BUCKET; bool head_done = false;
+    int64_t we = 0; /* end of the open window */
+
+    __device__ __forceinline__ SegWindows(const QueryP &q_, const ChunkP &ch_, uint32_t seg_, size_t e_, uint32_t series_)
+        : q(q_), ch(ch_), seg(seg_), e(e_), series(series_) {}
+    template <int NC> __device__ __forceinline__ void flush(const Part (&parts)[NC], bool final) {
+        if (cur_b == OG_NO_BUCKET) return;
+#pragma unroll
+        for (int c = 0; c < NC; c++) {
+            if (!head_done) store_part(ch.edges[c], e, parts[c]);
+            else if (final) store_part(ch.edges[c], e + 1, parts[c]);
+            else if (parts[c].ok) store_cell(ch, c, series, cur_b, parts[c]);
+        }
+        if (!head_done) { head_done = true; head_b = cur_b; }
+    }
+    /* an in-range row at time t: when t leaves the open window, that window is flushed and the partials start empty.
+     * false: t lies past the query's buckets (cannot happen on a validated shard), the walk ends */
+    template <int NC> __device__ __forceinline__ bool enter(int64_t t, Part (&parts)[NC]) {
+        if (cur_b != OG_NO_BUCKET && t < we) return true;
+        flush(parts, false);
+        cur_b = bucket_of(t, q.start, q.interval);
+        if (cur_b >= q.n_buckets) { report_err(ch.err, D_CORRUPT, seg); cur_b = OG_NO_BUCKET; return false; }
+        we = q.start + (int64_t)(cur_b + 1) * q.interval;
+#pragma unroll
+        for (int c = 0; c < NC; c++) parts[c] = part_empty();
+        return true;
+    }
+    /* after the row loop: the open window is the tail (or the head, when it is the only one) */
+    template <int NC> __device__ __forceinline__ void end(const Part (&parts)[NC]) {
+        const uint32_t last_b = cur_b;
+        const bool single = !head_done;
+        flush(parts, true);
+        ch.edge_bucket[e] = head_b;
+        ch.edge_bucket[e + 1] = (single || head_b == OG_NO_BUCKET) ? OG_NO_BUCKET : last_b;
+        if (head_b != OG_NO_BUCKET) ch.flags[1] = 1; /* edge windows written: k_fix_edges_fold has work */
+    }
+};
 
 /* ------------------------------------------------------------------------------------------------------------
  * shard open: row counts, codec support and framing validation (one thread per segment)
@@ -223,14 +271,6 @@ __global__ void k_filter_tile(DirP d, QueryP q, TileP tp) {
         keep = stack & 1;
     }
     tp.keep[idx] = keep;
-}
-
-/* where does a segment's partial for bucket b (w-th window of nwin) go */
-__device__ __forceinline__ void emit_window(const QueryP &q, const ChunkP &ch, uint32_t seg, uint32_t series, uint32_t b,
-                                            bool is_head, bool is_tail, int call, const Part &p) {
-    if (is_head) store_part(ch.edges[call], 2 * (size_t)(seg - ch.seg_begin), p);
-    else if (is_tail) store_part(ch.edges[call], 2 * (size_t)(seg - ch.seg_begin) + 1, p);
-    else if (p.ok) store_cell(ch, call, series, b, p);
 }
 
 /* step 3: one thread per segment walks its rows in time order (threads of a warp own consecutive segments and move row by row

@@ -534,6 +534,12 @@ void launch_multi(const QueryP &p, const DirP &d, const ChunkP &ch, uint32_t nse
     case 1: return launch_multi_c<1>(p, d, ch, nseg, st);
     case 2: return launch_multi_c<2>(p, d, ch, nseg, st);
     case 3: return launch_multi_c<3>(p, d, ch, nseg, st);
+#ifdef OG_WIDE_MULTI
+    case 5: return launch_multi_c<5>(p, d, ch, nseg, st);
+    case 6: return launch_multi_c<6>(p, d, ch, nseg, st);
+    case 7: return launch_multi_c<7>(p, d, ch, nseg, st);
+    case 8: return launch_multi_c<8>(p, d, ch, nseg, st);
+#endif
     default: return launch_multi_c<4>(p, d, ch, nseg, st);
     }
 }

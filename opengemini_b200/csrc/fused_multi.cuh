@@ -8,9 +8,9 @@
  * before it filters and reduces; here each column of the segment is a PULL iterator (ColIter, decode.cuh) and time comes from
  * a TimeIter, so a row's columns meet in registers: WHERE is evaluated on them (lib/binaryfilterfunc/functions.go:632
  * semantics: NULL never matches, ordered tests pass NaN), the surviving row is accumulated into the open window's partials,
- * and only window partials leave the thread (edges / per-series cells, the layout k_window_reduce and k_fused_cols write, so
- * k_fix_edges and the merges are shared).  Pages are read front to back, and consecutive 8-byte reads of one thread hit the
- * sector/line its previous read brought into L1: DRAM traffic stays at the page bytes.
+ * and only window partials leave the thread (edges / per-series cells through SegWindows; k_window_reduce and k_fused_cols
+ * write the same layout, so k_fix_edges and the merges are shared).  Pages are read front to back, and consecutive 8-byte
+ * reads of one thread hit the sector/line its previous read brought into L1: DRAM traffic stays at the page bytes.
  *
  * Replaces (for <= OG_MULTI_MAXC columns): readSegmentRecord (tssp_file.go:369) + decodeColumnData (reader.go:674) for every
  * codec the device knows + FilterByTime (reader.go:754) + FilterByField (reader.go:895-974, functions.go:632)
@@ -22,7 +22,14 @@
 
 namespace ogpu {
 
+/* Queries over more columns than this that k_fused_cols does not take run the materialise-tile path.  Building with
+ * -DOG_WIDE_MULTI (tools/build_variants.sh wide:"-DOG_WIDE_MULTI") serves them here instead, with an exact instance for
+ * each column count up to OG_MAX_COLS: the experiment behind the six-column row of DESIGN.md "Measured" (tools/bench_wide.py). */
+#ifdef OG_WIDE_MULTI
+#define OG_MULTI_MAXC OG_MAX_COLS
+#else
 #define OG_MULTI_MAXC 4
+#endif
 
 /* NCALL = number of calls (partials live in registers); SIMPLE = every call is count or sum (the shape configs[2] names): the
  * per-call switch of acc_row collapses to an add */
@@ -48,18 +55,7 @@ __global__ void __launch_bounds__(128) k_fused_multi(DirP d, QueryP q, ChunkP ch
         if (col[k].err != D_OK) { report_err(ch.err, col[k].err, seg); no_rows(); return; }
     }
     Part parts[NCALL];
-    uint32_t cur_b = OG_NO_BUCKET, head_b = OG_NO_BUCKET; bool head_done = false;
-    int64_t we = 0;
-    auto flush = [&](bool final) {
-        if (cur_b == OG_NO_BUCKET) return;
-#pragma unroll
-        for (int c = 0; c < NCALL; c++) {
-            if (!head_done) store_part(ch.edges[c], e, parts[c]);
-            else if (final) store_part(ch.edges[c], e + 1, parts[c]);
-            else if (parts[c].ok) store_cell(ch, (int)c, series, cur_b, parts[c]);
-        }
-        if (!head_done) { head_done = true; head_b = cur_b; }
-    };
+    SegWindows w(q, ch, seg, e, series);
     uint32_t r = 0;
     for (; r < rows; r++) {
         const int64_t t = ti.next();
@@ -68,14 +64,7 @@ __global__ void __launch_bounds__(128) k_fused_multi(DirP d, QueryP q, ChunkP ch
         for (int k = 0; k < NCOL; k++) { v[k] = 0; ok[k] = col[k].next(v[k]); } /* every column advances on every row, kept or not */
         if (t < q.tmin) continue;
         if (t > q.tmax) break;
-        if (cur_b == OG_NO_BUCKET || t >= we) {
-            flush(false);
-            cur_b = bucket_of(t, q.start, q.interval);
-            if (cur_b >= q.n_buckets) { report_err(ch.err, D_CORRUPT, seg); cur_b = OG_NO_BUCKET; break; } /* cannot happen on a validated shard */
-            we = q.start + (int64_t)(cur_b + 1) * q.interval;
-#pragma unroll
-            for (int c = 0; c < NCALL; c++) parts[c] = part_empty();
-        }
+        if (!w.enter(t, parts)) break;
         bool keep = true;
         if (q.n_filter == 1) { /* one compare term: no stack machine */
             const FilterP &f = q.filter[0];
@@ -122,11 +111,7 @@ __global__ void __launch_bounds__(128) k_fused_multi(DirP d, QueryP q, ChunkP ch
     }
     if (ti.err != D_OK) report_err(ch.err, ti.err, seg);
     for (int k = 0; k < NCOL; k++) if (col[k].err != D_OK) report_err(ch.err, col[k].err, seg);
-    const uint32_t last_b = cur_b;
-    const bool single = !head_done;
-    flush(true);
-    ch.edge_bucket[e] = head_b;
-    ch.edge_bucket[e + 1] = (single || head_b == OG_NO_BUCKET) ? OG_NO_BUCKET : last_b;
+    w.end(parts);
 }
 
 /* One column, no WHERE (og_stats.path 1, and the segments k_fused_il leaves over): the row loop of k_fused_multi without the
@@ -153,18 +138,7 @@ __global__ void __launch_bounds__(128) k_fused_segment(DirP d, QueryP q, ChunkP 
     col.init(d.data + d.page_off[pi], d.page_len[pi], q.col_type[0], rows);
     if (col.err != D_OK) { report_err(ch.err, col.err, seg); no_rows(); return; }
     Part parts[NC];
-    uint32_t cur_b = OG_NO_BUCKET, head_b = OG_NO_BUCKET; bool head_done = false;
-    int64_t we = 0;
-    auto flush = [&](bool final) {
-        if (cur_b == OG_NO_BUCKET) return;
-#pragma unroll
-        for (int c = 0; c < NC; c++) {
-            if (!head_done) store_part(ch.edges[c], e, parts[c]);
-            else if (final) store_part(ch.edges[c], e + 1, parts[c]);
-            else if (parts[c].ok) store_cell(ch, (int)c, series, cur_b, parts[c]);
-        }
-        if (!head_done) { head_done = true; head_b = cur_b; }
-    };
+    SegWindows w(q, ch, seg, e, series);
     uint32_t r = 0;
     auto walk = [&](auto kind) {
         col.kind = decltype(kind)::value; /* a constant from here on: value() reduces to this codec's case */
@@ -174,14 +148,7 @@ __global__ void __launch_bounds__(128) k_fused_segment(DirP d, QueryP q, ChunkP 
             const bool ok = col.next(v);
             if (t < q.tmin) continue;
             if (t > q.tmax) break;
-            if (cur_b == OG_NO_BUCKET || t >= we) {
-                flush(false);
-                cur_b = bucket_of(t, q.start, q.interval);
-                if (cur_b >= q.n_buckets) { report_err(ch.err, D_CORRUPT, seg); cur_b = OG_NO_BUCKET; break; } /* cannot happen on a validated shard */
-                we = q.start + (int64_t)(cur_b + 1) * q.interval;
-#pragma unroll
-                for (int c = 0; c < NC; c++) parts[c] = part_empty();
-            }
+            if (!w.enter(t, parts)) break;
             if (ok) {
 #pragma unroll
                 for (int c = 0; c < NC; c++) acc_row(q.calls[c].func, q.calls[c].type, parts[c], v, t);
@@ -207,12 +174,7 @@ __global__ void __launch_bounds__(128) k_fused_segment(DirP d, QueryP q, ChunkP 
     }
     if (ti.err != D_OK) report_err(ch.err, ti.err, seg);
     if (col.err != D_OK) report_err(ch.err, col.err, seg);
-    const uint32_t last_b = cur_b;
-    const bool single = !head_done;
-    flush(true);
-    ch.edge_bucket[e] = head_b;
-    ch.edge_bucket[e + 1] = (single || head_b == OG_NO_BUCKET) ? OG_NO_BUCKET : last_b;
-    if (head_b != OG_NO_BUCKET) ch.flags[1] = 1; /* edge windows written: k_fix_edges_fold has work */
+    w.end(parts);
 }
 
 } // namespace ogpu
