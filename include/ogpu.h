@@ -31,6 +31,9 @@
  *                            chunkdata_builder.go:65 EncodeTime (downsample / compaction re-encode).
  *   og_downsample            engine/record_plan.go:494-830 + engine/immutable/stream_downsample.go:454-600: one column of a shard
  *                            -> per-series window aggregates -> re-encoded pages and their directory, in one call.
+ *   og_downsample_shard      the same for every field of a shard under a per-type call list (services/downsample/functions.go:42-111,
+ *                            executor/schema.go:1448-1475, engine/record_plan.go:256-420,494-830): <call>_<field> columns,
+ *                            null cells where a field had no value in a kept window.
  *   og_shard_synth           test/bench tooling: builds a synthetic shard directly in HBM with the encode kernels
  *                            (same bytes the oracle's restated encoders produce; see tests/test_gpu_parity.py::test_synth_pages_byte_exact).
  *
@@ -384,6 +387,40 @@ OG_API int og_encode_pages(int32_t type, int32_t is_time, const void *d_values, 
  * the host for a file writer. ---- */
 typedef struct og_downsampled og_downsampled;
 OG_API int og_downsample(og_shard *s, uint32_t column, int64_t interval, int64_t tmin, int64_t tmax, og_downsampled **out);
+
+/* ---- downsample a whole shard under a per-type policy (csrc/downsample.cu): what the reference's downsample task writes for one
+ * shard of one measurement.  Replaces services/downsample/functions.go:42-111 (initDownSampleSchema: DownSamplePolicyInfo.GetCalls()
+ * gives a call list per field type, applied to every field of that type; fields of a type without a list are dropped;
+ * downSampleExprGen names each column <call>_<field>), executor/schema.go:1448-1475 (the output schema, addPrefix = true; count
+ * is an integer column, the other calls keep the source type), engine/record_plan.go:256-420 (FieldIter / ChunkMetaByField read
+ * a series one field at a time) and :494-830 (FileSequenceAggregator reduces per series and window, WriteIntoStorageTransform
+ * writes the fields of a series against one time column).
+ *   Calls by type: float, int: all six.  bool: count, min, max, first, last (sum is OG_E_INVAL: no boolean sum reducer).
+ *   string: count only (any other call is OG_E_UNSUPPORTED: string values are never decoded on the device).  A type listed twice,
+ *   a function outside OG_AGG_*, or a function listed twice in one list is OG_E_INVAL.  A type with an empty list is a type
+ *   without a list.  A range whose first or last window is clamped at the int64 time limits is refused as og_query_create
+ *   refuses it.
+ *   Columns: one per (call, field) with calls, sorted by name; `og_shard_synth` shards name their fields f<c>.
+ *   Rows: a series has one row per window in which ANY of its output cells is non-null, timed at the window start; a cell whose
+ *   field had no non-null value in that window is null, and its page carries a bitmap.  (The reference gap-fills each field's
+ *   windows with null rows across the series' time range, AppendRecWithNilRows record_plan.go:1234-1260, and so also writes rows
+ *   that are null in every column; these are dropped here, as og_downsample drops empty windows.  DESIGN.md "Deviations".)
+ *   Segments: 1000 rows; a series without rows in range has none.
+ * The result is an ordinary og_downsampled handle: og_downsampled_desc / _export / _free serve it. ---- */
+typedef struct og_downsample_ops {
+    int32_t type;          /* OG_TYPE_* */
+    uint32_t n_funcs;
+    const int32_t *funcs;  /* [n_funcs] OG_AGG_* */
+} og_downsample_ops;
+typedef struct og_downsample_desc {
+    int64_t interval, tmin, tmax;   /* window length (> 0) and inclusive time range, as og_downsample takes them */
+    uint32_t n_types;
+    const og_downsample_ops *ops;   /* [n_types] at most one entry per type; a type without an entry drops its fields */
+} og_downsample_desc;
+OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_downsampled **out);
+/* wall-clock milliseconds of og_downsample_shard's phases: [0] the per-column queries, [1] k_dsx_keep + scan + k_dsx_scatter,
+ * [2] page encoding, [3] directory assembly and the output copy.  All zero for og_downsample results. */
+OG_API int og_downsampled_timing(const og_downsampled *d, double phase_ms[4]);
 OG_API int og_downsampled_desc(const og_downsampled *d, og_shard_desc *desc, uint64_t *rows /* may be NULL */);
 OG_API int og_downsampled_export(const og_downsampled *d, uint8_t *host_data /* desc->data_len bytes */);
 OG_API void og_downsampled_free(og_downsampled *d);

@@ -96,6 +96,15 @@ class ShardLayout(C.Structure):
     _fields_ = [("data_len", C.c_uint64), ("n_series", C.c_uint32), ("n_segments", C.c_uint32), ("n_columns", C.c_uint32)]
 
 
+class DownsampleOps(C.Structure):
+    _fields_ = [("type", C.c_int32), ("n_funcs", C.c_uint32), ("funcs", i32p)]
+
+
+class DownsampleDesc(C.Structure):
+    _fields_ = [("interval", C.c_int64), ("tmin", C.c_int64), ("tmax", C.c_int64), ("n_types", C.c_uint32),
+                ("ops", C.POINTER(DownsampleOps))]
+
+
 class MergeInfo(C.Structure):
     _fields_ = [("n_files", C.c_uint32), ("n_out_of_order_files", C.c_uint32), ("series_merged", C.c_uint64),
                 ("out_of_order_rows", C.c_uint64), ("rows_replaced", C.c_uint64), ("rows_after_merge", C.c_uint64),
@@ -111,6 +120,7 @@ EXPORTS = [
     "og_shard_synth", "og_shard_layout_get", "og_shard_export", "og_encode_pages",
     "og_release_cached_memory", "og_comm_unique_id", "og_comm_init_rank", "og_comm_destroy", "og_comm_info", "og_comm_allreduce_f64", "og_query_allreduce",
     "og_downsample", "og_downsampled_desc", "og_downsampled_export", "og_downsampled_free",
+    "og_downsample_shard", "og_downsampled_timing",
     "og_tssp_parse", "og_tssp_desc", "og_tssp_measurement", "og_tssp_time_range", "og_tssp_free",
     "og_shard_open_files", "og_shard_merge_info",
 ]
@@ -157,6 +167,8 @@ def lib():
     L.og_query_merge_dense.argtypes = [C.c_void_p, C.POINTER(DenseView)]
     L.og_decode_segment.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(RecordView)]
     L.og_downsample.argtypes = [C.c_void_p, C.c_uint32, C.c_int64, C.c_int64, C.c_int64, C.POINTER(C.c_void_p)]
+    L.og_downsample_shard.argtypes = [C.c_void_p, C.POINTER(DownsampleDesc), C.POINTER(C.c_void_p)]
+    L.og_downsampled_timing.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
     L.og_downsampled_desc.argtypes = [C.c_void_p, C.POINTER(ShardDesc), C.POINTER(C.c_uint64)]
     L.og_downsampled_export.argtypes = [C.c_void_p, C.c_void_p]
     L.og_downsampled_free.argtypes = [C.c_void_p]

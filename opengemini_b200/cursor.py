@@ -190,6 +190,21 @@ class Shard:
         L.check(L.lib().og_downsample(self.h, column, interval, tmin, tmax, C.byref(h)), "og_downsample")
         return Downsampled(h.value)
 
+    def downsample_shard(self, interval, tmin, tmax, ops):
+        """og_downsample_shard: every field under a per-type call list -> <call>_<field> columns with null cells, in one library
+        call.  ops: {OG type: [call name or OG_AGG_* value, ...]}; a type without an entry drops its fields."""
+        entries = list(ops.items())
+        arr = (L.DownsampleOps * max(1, len(entries)))()
+        keep = []
+        for i, (typ, funcs) in enumerate(entries):
+            f = (C.c_int32 * max(1, len(funcs)))(*[_FUNCS[x] if isinstance(x, str) else int(x) for x in funcs])
+            keep.append(f)
+            arr[i].type, arr[i].n_funcs, arr[i].funcs = int(typ), len(funcs), C.cast(f, L.i32p)
+        d = L.DownsampleDesc(int(interval), int(tmin), int(tmax), len(entries), arr)
+        h = C.c_void_p()
+        L.check(L.lib().og_downsample_shard(self.h, C.byref(d), C.byref(h)), "og_downsample_shard")
+        return Downsampled(h.value)
+
     def decode_segment(self, seg, descending=False):
         rv = L.RecordView()
         L.check(L.lib().og_decode_segment_ex(self.h, seg, 1 if descending else 0, C.byref(rv)), "og_decode_segment_ex")
@@ -225,6 +240,23 @@ class Downsampled:
         out = np.empty(max(1, self.desc.data_len), np.uint8)
         L.check(L.lib().og_downsampled_export(self.h, out.ctypes.data), "og_downsampled_export")
         return out[:self.desc.data_len]
+
+    def timing(self):
+        """Milliseconds of og_downsample_shard's phases (zeros for og_downsample results)."""
+        ms = (C.c_double * 4)()
+        L.check(L.lib().og_downsampled_timing(self.h, ms), "og_downsampled_timing")
+        return dict(queries=ms[0], keep_scatter=ms[1], encode=ms[2], assembly=ms[3])
+
+    def columns(self):
+        """[(name, type, page_off, page_len)] of the field columns, then the time column's (page_off, page_len)."""
+        d, ng = self.desc, self.desc.n_segments
+        cols = [(d.columns[c].name.decode(), int(d.columns[c].type),
+                 np.ctypeslib.as_array(d.columns[c].page_off, shape=(ng,)).copy() if ng else np.empty(0, np.uint64),
+                 np.ctypeslib.as_array(d.columns[c].page_len, shape=(ng,)).copy() if ng else np.empty(0, np.uint32))
+                for c in range(d.n_columns)]
+        t = (np.ctypeslib.as_array(d.time_page_off, shape=(ng,)).copy() if ng else np.empty(0, np.uint64),
+             np.ctypeslib.as_array(d.time_page_len, shape=(ng,)).copy() if ng else np.empty(0, np.uint32))
+        return cols, t
 
     def close(self):
         if self.h:

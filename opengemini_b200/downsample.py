@@ -8,6 +8,9 @@ torch is only used to reshape device arrays between the two calls.  Output colum
 downsample schema: min_, max_, sum_, count_, first_, last_ of the source field, window start as the row time, empty windows
 dropped (lib/record/record.go:1298-1365 TransIntervalRec2Rec).
 
+downsample_shard() is the whole-shard form behind one library call (og_downsample_shard): every field under the policy's call list
+for its type, <call>_<field> columns, null cells where a field had no value in a kept window.
+
 No CPU fallback: every step runs through libogpu.so.
 """
 import ctypes as C
@@ -15,7 +18,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib as L
-from .cursor import AggQuery
+from .cursor import AggQuery, device_view
 
 OUT_CALLS = ("min", "max", "sum", "count", "first", "last")
 ROWS_PER_SEGMENT = 1000  # lib/util/util.go:72
@@ -86,3 +89,32 @@ def downsample(shard, column, interval, tmin, tmax, col_type=L.TYPE_FLOAT):
                     seg_tmin=seg_tmin, seg_tmax=seg_tmax, sids=np.arange(1, ns + 1, dtype=np.uint64), rows=int(rows_s.sum()))
     finally:
         q.close()
+
+
+def downsample_shard(shard, interval, tmin, tmax, ops):
+    """Every field of `shard` under a per-type policy in one library call (og_downsample_shard): ops = {OG type: [call, ...]},
+    e.g. {L.TYPE_FLOAT: ["min", "max", "sum", "count", "first", "last"], L.TYPE_BOOL: ["count", "last"]}.  Fields of a type
+    without an entry are dropped; each output column is named <call>_<field>; a series keeps a window where any of its
+    output cells is non-null, and cells without a value are null (their pages carry a bitmap).
+
+    Returns the dict downsample() returns (data: uint8 torch tensor on the device, with the 1024-byte tail readers need), plus
+    names=[column names in schema order] and timing={phase: ms}."""
+    import torch
+
+    ds = shard.downsample_shard(interval, tmin, tmax, ops)
+    try:
+        d = ds.desc
+        columns, (tpo, tpl) = ds.columns()
+        ns, ng = d.n_series, d.n_segments
+        dev = torch.device("cuda", torch.cuda.current_device())
+        # the handle owns the pages: copy them (device to device) into a tensor that outlives it
+        data = device_view(C.cast(d.data, C.c_void_p).value, d.data_len + 1024, "|u1", dev).clone()
+        torch.cuda.synchronize(dev)
+        return dict(data=data, data_len=int(d.data_len), columns=columns, names=[c[0] for c in columns], time_page_off=tpo,
+                    time_page_len=tpl, series_seg_begin=np.ctypeslib.as_array(d.series_seg_begin, shape=(ns + 1,)).copy(),
+                    seg_tmin=np.ctypeslib.as_array(d.seg_tmin, shape=(ng,)).copy() if ng else np.empty(0, np.int64),
+                    seg_tmax=np.ctypeslib.as_array(d.seg_tmax, shape=(ng,)).copy() if ng else np.empty(0, np.int64),
+                    sids=np.ctypeslib.as_array(d.sids, shape=(ns,)).copy() if ns else np.empty(0, np.uint64), rows=int(ds.rows),
+                    timing=ds.timing())
+    finally:
+        ds.close()
