@@ -34,6 +34,9 @@
  *   og_downsample_shard      the same for every field of a shard under a per-type call list (services/downsample/functions.go:42-111,
  *                            executor/schema.go:1448-1475, engine/record_plan.go:256-420,494-830): <call>_<field> columns,
  *                            null cells where a field had no value in a kept window.
+ *   og_shard_write_tssp      engine/immutable/msbuilder.go:1248-1303,1355-1433 (MsBuilder.WriteData / Flush), chunkdata_builder_ts.go:37-82
+ *                            (EncodeChunk: per column [crc32][pages]), pre_aggregation.go (the pre-agg blob of every ColumnMeta): an
+ *                            open shard -> the bytes of one TSSP file, chunks laid out and checksummed on the device.
  *   og_shard_synth           test/bench tooling: builds a synthetic shard directly in HBM with the encode kernels
  *                            (same bytes the oracle's restated encoders produce; see tests/test_gpu_parity.py::test_synth_pages_byte_exact).
  *
@@ -424,6 +427,40 @@ OG_API int og_downsampled_timing(const og_downsampled *d, double phase_ms[4]);
 OG_API int og_downsampled_desc(const og_downsampled *d, og_shard_desc *desc, uint64_t *rows /* may be NULL */);
 OG_API int og_downsampled_export(const og_downsampled *d, uint8_t *host_data /* desc->data_len bytes */);
 OG_API void og_downsampled_free(og_downsampled *d);
+
+/* ---- an open shard as one TSSP file (csrc/tssp_write.cu, csrc/tssp.cpp).  Replaces, for data that is already on the device,
+ * MsBuilder.WriteData / Flush (engine/immutable/msbuilder.go:1248-1303,1355-1433), TsChunkDataImp.EncodeChunk
+ * (chunkdata_builder_ts.go:37-82), ChunkDataBuilder.EncodeTime (chunkdata_builder.go:65-114) and the pre-aggregation builders
+ * (pre_aggregation.go).  Works on any og_shard: opened from a description or a file, synthesised, merged from a file set, or a
+ * downsample result reopened in place (og_downsampled_desc -> og_shard_open).  The file is version 2, attached layout,
+ * ChunkMetaCompressNone: header | chunks | chunk-meta blocks | meta index | bloom filter | id-time | trailer | footer, and
+ * og_tssp_parse -> og_shard_open of its bytes gives back the shard's series, segments and pages.
+ *   Pages are copied byte for byte; only pages the directory references are written (a merged shard's rewritten source pages
+ *   stay behind; pages that were Snappy in the source were transcoded to raw pages at open, and those are written).  Every ColumnMeta carries the pre-aggregation blob of the column's rows as the reference's builders compute it
+ *   (min / max with the time of their first occurrence, sum in row order, count; DESIGN.md lists what differs from the query
+ *   reducers), every column of a chunk is prefixed by the CRC32 (IEEE) of its pages.
+ *   A series without segments has no chunk.  A column whose page_len is 0 in every segment of a series is left out of that
+ *   series' ChunkMeta, as the reference writes a series that lacks a field; all-null pages are pages and are listed.
+ * Refused: an empty series range, a range none of whose series holds rows, series ids that are zero or not strictly ascending
+ * (msbuilder.go:1252-1256) — OG_E_INVAL; a series with more than 65535 segments, a file above 8 GiB (engine/immutable/config.go:24-31,
+ * lib/util/util.go:83), a column present in only some segments of a series, id-time values that the reference would encode
+ * with zstd — OG_E_UNSUPPORTED, with text that says to narrow the series range where that helps; a page that does not decode —
+ * OG_E_CORRUPT. ---- */
+typedef struct og_tssp_write_desc {
+    const char *measurement;            /* TableStat.name */
+    uint32_t series_begin, series_end;  /* half-open range of the shard's series; 0,0 = all.  How a caller splits a shard that
+                                           exceeds the per-file limits into several files */
+    uint32_t flags;                     /* 0 */
+} og_tssp_write_desc;
+typedef struct og_tssp_image og_tssp_image;
+OG_API int og_shard_write_tssp(og_shard *s, const og_tssp_write_desc *d, og_tssp_image **out);
+OG_API int og_tssp_image_size(const og_tssp_image *f, uint64_t *bytes);
+/* the whole file into `host` (og_tssp_image_size bytes): one device-to-host copy of the chunk region, the rest from host memory */
+OG_API int og_tssp_image_export(const og_tssp_image *f, uint8_t *host);
+/* wall-clock milliseconds of og_shard_write_tssp's phases: [0] pre-aggregation (k_preagg), [1] layout scan + k_tssp_gather +
+ * k_tssp_crc_fold, [2] metadata to the host, [3] host assembly of everything behind the chunks */
+OG_API int og_tssp_image_timing(const og_tssp_image *f, double phase_ms[4]);
+OG_API void og_tssp_image_free(og_tssp_image *f);
 
 #ifdef __cplusplus
 }

@@ -5,6 +5,6 @@ This package only holds the host-side bindings; aggregation and decoding never r
 (the bindings only slice the records the library returns).
 """
 from . import _lib  # noqa: F401
-from .cursor import AggQuery, Comm, ScanCursor, Shard  # noqa: F401
+from .cursor import AggQuery, Comm, ScanCursor, Shard, write_tssp  # noqa: F401
 
-__all__ = ["Shard", "AggQuery", "ScanCursor", "Comm", "_lib"]
+__all__ = ["Shard", "AggQuery", "ScanCursor", "Comm", "write_tssp", "_lib"]

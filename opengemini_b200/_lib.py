@@ -112,6 +112,10 @@ class MergeInfo(C.Structure):
                 ("merge_ms", C.c_double)]
 
 
+class TsspWriteDesc(C.Structure):
+    _fields_ = [("measurement", C.c_char_p), ("series_begin", C.c_uint32), ("series_end", C.c_uint32), ("flags", C.c_uint32)]
+
+
 # every symbol include/ogpu.h declares (checked by tests/test_abi.py against the header text)
 EXPORTS = [
     "og_init", "og_device_count", "og_strerror", "og_last_error", "og_version", "og_shard_open", "og_shard_close",
@@ -123,6 +127,7 @@ EXPORTS = [
     "og_downsample_shard", "og_downsampled_timing",
     "og_tssp_parse", "og_tssp_desc", "og_tssp_measurement", "og_tssp_time_range", "og_tssp_free",
     "og_shard_open_files", "og_shard_merge_info",
+    "og_shard_write_tssp", "og_tssp_image_size", "og_tssp_image_export", "og_tssp_image_timing", "og_tssp_image_free",
 ]
 
 _lib = None
@@ -180,6 +185,12 @@ def lib():
     L.og_tssp_time_range.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.og_tssp_free.argtypes = [C.c_void_p]
     L.og_tssp_free.restype = None
+    L.og_shard_write_tssp.argtypes = [C.c_void_p, C.POINTER(TsspWriteDesc), C.POINTER(C.c_void_p)]
+    L.og_tssp_image_size.argtypes = [C.c_void_p, u64p]
+    L.og_tssp_image_export.argtypes = [C.c_void_p, C.c_void_p]
+    L.og_tssp_image_timing.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+    L.og_tssp_image_free.argtypes = [C.c_void_p]
+    L.og_tssp_image_free.restype = None
     L.og_decode_segment_ex.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(RecordView)]
     L.og_decode_column_device.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
     L.og_shard_synth.argtypes = [C.POINTER(SynthDesc), C.POINTER(C.c_void_p)]

@@ -1,7 +1,8 @@
 /*
- * tssp.cpp — the TSSP container, read side: file bytes -> og_shard_desc (the flattened ChunkMeta directory og_shard_open
- * takes).  Host code only: the container is a few bytes of metadata per segment, walked once per file; the pages it points
- * at are what the GPU reads.
+ * tssp.cpp — the TSSP container.  Read side: file bytes -> og_shard_desc (the flattened ChunkMeta directory og_shard_open
+ * takes).  Write side (tssp_build_tail, at the end of the file): everything of a file that follows its chunks, for
+ * og_shard_write_tssp (tssp_write.cu lays out and checksums the chunks on the device).  Host code only: the container is a few
+ * bytes of metadata per segment, walked once per file; the pages it points at are what the GPU reads and writes.
  *
  * What the reference does on this path (engine/immutable):
  *   file     = "53ac2021" | u64 BE version=2 | chunks | chunk-meta blocks | meta index | bloom | id-time | trailer | footer
@@ -22,6 +23,7 @@
  * (object-store) files.  The per-column CRC32 is not verified: pages are validated structurally on the device at og_shard_open.
  */
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <map>
 #include <memory>
@@ -29,6 +31,7 @@
 #include <vector>
 
 #include "../../include/ogpu.h"
+#include "tssp_write.h"
 
 namespace ogpu { void set_error(const char *fmt, ...); }
 using ogpu::set_error;
@@ -196,3 +199,194 @@ OG_API int og_tssp_time_range(const og_tssp *f, int64_t *min_time, int64_t *max_
 OG_API void og_tssp_free(og_tssp *f) { delete f; }
 
 } // extern "C"
+
+/* =============================================== write side ===============================================
+ * What MsBuilder writes behind the chunks (engine/immutable):
+ *   ChunkMeta.marshal / ColumnMeta.marshal     tssp_file_meta.go:566-581,228-246; pre-agg blobs pre_aggregation.go marshal()
+ *   chunk-meta blocks                          a block closes after 512 metas or once it holds >= 256 KiB (msbuilder.go:348-364,
+ *                                              lib/util/util.go:75-76), followed by the u32 start offsets of its metas (:1481-1500)
+ *   MetaIndex                                  first sid, time range, offset, count, size of each block (tssp_file_meta.go:769-778)
+ *   bloom filter                               msbuilder.go:1336-1353 genBloomFilter over lib/util/lifted/influxdb/pkg/bloom
+ *   id-time section                            sequencer.go:332-390 IdTimePairs.Marshal(encTimes = true)
+ *   trailer, footer                            trailer.go:58-66, table_stat.go:35-51,125-148, msbuilder.go:1409-1425
+ */
+namespace {
+
+struct Wr { /* big-endian appender */
+    std::vector<uint8_t> &b;
+    void u8(uint32_t v) { b.push_back((uint8_t)v); }
+    void u16(uint32_t v) { b.push_back((uint8_t)(v >> 8)); b.push_back((uint8_t)v); }
+    void u32(uint32_t v) { for (int i = 3; i >= 0; i--) b.push_back((uint8_t)(v >> (8 * i))); }
+    void u64(uint64_t v) { for (int i = 7; i >= 0; i--) b.push_back((uint8_t)(v >> (8 * i))); }
+    void i64(int64_t v) { u64(((uint64_t)v << 1) ^ (uint64_t)(v >> 63)); } /* zig-zag, lib/numberenc/number.go:156-160 */
+    void bytes(const void *p, size_t n) { const uint8_t *q = (const uint8_t *)p; b.insert(b.end(), q, q + n); }
+};
+
+/* IntegerPreAgg / FloatPreAgg / BooleanPreAgg / StringPreAgg / TimePreAgg .marshal() with ChunkMetaCompressNone */
+void put_preagg(Wr &w, int type, bool is_time, const ogpu::PreAggCell &c) {
+    if (is_time) { w.u16(4); w.u32((uint32_t)c.count); return; }
+    switch (type) {
+    case OG_TYPE_STRING: w.u16(8); w.i64(c.count); return;
+    case OG_TYPE_BOOL: w.u16(26); w.i64(c.count); w.i64(c.mint); w.i64(c.maxt); w.u8((uint32_t)c.minv); w.u8((uint32_t)c.maxv); return;
+    case OG_TYPE_FLOAT:
+        if (c.count == 1) { w.u16(16); w.u64(c.minv); w.i64(c.mint); return; }
+        w.u16(48); w.u64(c.minv); w.u64(c.maxv); w.i64(c.mint); w.i64(c.maxt); w.u64(c.sum); w.i64(c.count); return;
+    default: /* OG_TYPE_INT */
+        if (c.count == 1) { w.u16(16); w.i64((int64_t)c.minv); w.i64(c.mint); return; }
+        w.u16(48); w.i64((int64_t)c.minv); w.i64((int64_t)c.maxv); w.i64(c.mint); w.i64(c.maxt); w.i64((int64_t)c.sum); w.i64(c.count); return;
+    }
+}
+
+/* xxHash64, seed 0, of eight bytes (github.com/cespare/xxhash/v2 Sum64, the hash of the reference's bloom filter) */
+uint64_t xxh64_8(const uint8_t *p) {
+    const uint64_t P1 = 11400714785074694791ull, P2 = 14029467366897019727ull, P3 = 1609587929392839161ull, P4 = 9650029242287828579ull, P5 = 2870177450012600261ull;
+    auto rotl = [](uint64_t x, int r) { return (x << r) | (x >> (64 - r)); };
+    uint64_t k = 0; for (int i = 7; i >= 0; i--) k = (k << 8) | p[i];
+    uint64_t h = P5 + 8;
+    h ^= rotl(k * P2, 31) * P1;
+    h = rotl(h, 27) * P1 + P4;
+    h ^= h >> 33; h *= P2; h ^= h >> 29; h *= P3; h ^= h >> 32;
+    return h;
+}
+
+/* genBloomFilter: bloom.Estimate(n, 0.08), byte size rounded up to a power of two (at least 8), keys = big-endian sid */
+void bloom_of(const std::vector<uint64_t> &sids, std::vector<uint8_t> &bits, uint64_t &m, uint64_t &k) {
+    const double n = (double)sids.size(), ln2 = std::log(2.0);
+    m = (uint64_t)std::ceil(-1.0 * n * std::log(0.08) / (ln2 * ln2));
+    k = (uint64_t)std::ceil(ln2 * (double)m / n);
+    uint64_t nb = 8; while (nb < (m + 7) / 8) nb *= 2;
+    bits.assign(nb, 0);
+    const uint64_t mask = nb * 8 - 1;
+    for (uint64_t sid : sids) {
+        uint8_t key[8]; for (int i = 0; i < 8; i++) key[i] = (uint8_t)(sid >> (56 - 8 * i));
+        const uint64_t h0 = xxh64_8(key);
+        key[7] = 0; /* Filter.hash: the second hash is of the key with its last byte cleared */
+        const uint64_t h1 = xxh64_8(key);
+        for (uint64_t i = 0; i < k; i++) { const uint64_t loc = (h0 + h1 * i) & mask; bits[loc >> 3] |= (uint8_t)(1u << (loc & 7)); }
+    }
+}
+
+/* lib/encoding/int.go:66-212 Integer.Encoding: raw below three values, else zig-zag deltas as const-delta or Simple8b
+ * (simple8b/encoding.go:350-473 EncodeAll; selectors 0/1 only when every remaining value is 1).  false where the reference falls
+ * to zstd. */
+bool int_block(const int64_t *v, size_t n, Wr &w) {
+    auto zz = [](int64_t x) { return ((uint64_t)x << 1) ^ (uint64_t)(x >> 63); };
+    if (n < 3) { w.u8(0x40); w.u32((uint32_t)(8 * n)); for (size_t i = 0; i < n; i++) w.u64(zz(v[i])); return true; }
+    std::vector<uint64_t> d(n);
+    d[0] = zz(v[0]);
+    for (size_t i = 1; i < n; i++) d[i] = zz((int64_t)((uint64_t)v[i] - (uint64_t)v[i - 1]));
+    bool is_const = true, is_s8b = true;
+    for (size_t i = 1; i < n; i++) { if (i >= 2 && d[i] != d[i - 1]) is_const = false; if (d[i] > (1ull << 60) - 1) is_s8b = false; }
+    auto uvarint = [&](uint64_t x) { while (x >= 0x80) { w.u8((uint32_t)(x & 0x7f) | 0x80); x >>= 7; } w.u8((uint32_t)x); };
+    if (is_const) { w.u8(0x10); w.u64(d[0]); uvarint(d[1]); uvarint(n - 1); return true; }
+    if (!is_s8b) return false;
+    static const unsigned N[16] = {240, 120, 60, 30, 20, 15, 12, 10, 8, 7, 6, 5, 4, 3, 2, 1}, B[16] = {0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 10, 12, 15, 20, 30, 60};
+    std::vector<uint64_t> words;
+    size_t ones_from = n; /* d[ones_from..] are all 1 */
+    while (ones_from > 1 && d[ones_from - 1] == 1) ones_from--;
+    for (size_t i = 1; i < n;) {
+        int sel = 0;
+        for (; sel < 16; sel++) {
+            if (n - i < N[sel]) continue;
+            bool ok = true;
+            if (B[sel] == 0) ok = i >= ones_from;
+            else for (unsigned k = 0; k < N[sel] && ok; k++) ok = d[i + k] <= (1ull << B[sel]) - 1;
+            if (ok) break;
+        }
+        if (sel == 16) return false; /* unreachable: selector 15 packs any one value below 2^60 */
+        uint64_t word = (uint64_t)sel << 60;
+        if (B[sel]) for (unsigned k = 0; k < N[sel]; k++) word |= d[i + k] << (k * B[sel]);
+        words.push_back(word); i += N[sel];
+    }
+    w.u8(0x20); w.u32((uint32_t)words.size() + 1); w.u32((uint32_t)n); w.u64(d[0]);
+    for (uint64_t x : words) w.u64(x);
+    return true;
+}
+
+} // namespace
+
+int ogpu::tssp_build_tail(const TsspTailIn &in, std::vector<uint8_t> &out) {
+    out.clear();
+    Wr w{out};
+    const uint32_t nc1 = in.n_cols1;
+    const uint64_t meta_off = in.chunk_off[in.n_series];
+    struct Item { uint64_t id; int64_t tmin, tmax; uint64_t off; uint32_t count, size; };
+    std::vector<Item> items;
+    std::vector<uint32_t> starts;
+    std::vector<uint64_t> ids; std::vector<int64_t> rows, last_times;
+    size_t block_begin = 0;
+    int64_t file_tmin = INT64_MAX, file_tmax = INT64_MIN;
+    Item cur{};
+    auto close_block = [&]() { /* SwitchChunkMeta */
+        for (uint32_t s : starts) w.u32(s);
+        cur.size = (uint32_t)(out.size() - block_begin);
+        items.push_back(cur);
+        starts.clear(); block_begin = out.size(); cur = Item{};
+    };
+    for (uint32_t i = 0; i < in.n_series; i++) {
+        const uint32_t g0 = in.seg_begin[i], nseg = in.seg_begin[i + 1] - g0;
+        if (nseg == 0) continue; /* a series without rows has no chunk */
+        const int64_t tmin = in.seg_tmin[g0], tmax = in.seg_tmax[g0 + nseg - 1]; /* ChunkMeta.MinMaxTime of a time-sorted chunk */
+        if (cur.count == 0) { cur.id = in.sids[i]; cur.tmin = tmin; cur.tmax = tmax; cur.off = meta_off + block_begin; }
+        cur.tmin = std::min(cur.tmin, tmin); cur.tmax = std::max(cur.tmax, tmax);
+        file_tmin = std::min(file_tmin, tmin); file_tmax = std::max(file_tmax, tmax);
+        starts.push_back((uint32_t)(out.size() - block_begin));
+        uint32_t ncol = 0;
+        for (uint32_t c = 0; c < nc1; c++) ncol += in.col_present[(size_t)i * nc1 + c];
+        w.u64(in.sids[i]); w.i64((int64_t)in.chunk_off[i]); w.u32((uint32_t)(in.chunk_off[i + 1] - in.chunk_off[i])); w.u32(ncol); w.u32(nseg);
+        for (uint32_t s = 0; s < nseg; s++) { w.i64(in.seg_tmin[g0 + s]); w.i64(in.seg_tmax[g0 + s]); }
+        for (uint32_t c = 0; c < nc1; c++) {
+            if (!in.col_present[(size_t)i * nc1 + c]) continue;
+            const bool is_time = c + 1 == nc1;
+            const std::string name = is_time ? "time" : in.col_names[c];
+            const int type = is_time ? OG_TYPE_INT : in.col_types[c];
+            w.u16((uint32_t)name.size()); w.bytes(name.data(), name.size()); w.u8((uint32_t)type);
+            put_preagg(w, type, is_time, in.cells[(size_t)i * nc1 + c]);
+            for (uint32_t s = 0; s < nseg; s++) { const size_t pi = (size_t)c * in.n_segments + g0 + s; w.i64((int64_t)in.page_off[pi]); w.u32(in.page_len[pi]); }
+        }
+        ids.push_back(in.sids[i]); rows.push_back(in.cells[(size_t)i * nc1 + nc1 - 1].count); last_times.push_back(tmax);
+        cur.count++;
+        if (out.size() - block_begin >= 256 * 1024 || cur.count >= 512) close_block(); /* needSwitchChunkMeta */
+    }
+    if (ids.empty()) { set_error("no series of the range holds rows: a TSSP file cannot be empty"); return OG_E_INVAL; }
+    if (cur.count) close_block();
+    const uint64_t index_size = out.size();
+    for (const Item &m : items) { w.u64(m.id); w.i64(m.tmin); w.i64(m.tmax); w.i64((int64_t)m.off); w.u32(m.count); w.u32(m.size); }
+    const uint64_t mi_size = out.size() - index_size;
+    std::vector<uint8_t> bloom; uint64_t bloom_m, bloom_k;
+    bloom_of(ids, bloom, bloom_m, bloom_k);
+    w.bytes(bloom.data(), bloom.size());
+    /* id-time: blocks of 2000 series, each [u32 count] then the sids, row counts and last times as length-prefixed integer blocks */
+    const uint64_t idtime_begin = out.size();
+    const uint32_t n = (uint32_t)ids.size(), per = 2000, blocks = (n + per - 1) / per;
+    w.u32(n); w.u32(blocks);
+    for (uint32_t b = 0; b < blocks; b++) {
+        const uint32_t at = b * per, cnt = std::min(per, n - at);
+        w.u32(cnt);
+        const int64_t *arr[3] = {(const int64_t *)ids.data() + at, rows.data() + at, last_times.data() + at};
+        for (int a = 0; a < 3; a++) {
+            const size_t pos = out.size();
+            w.u32(0);
+            if (!int_block(arr[a], cnt, w)) {
+                set_error("id-time section: the %s of series %u.. need the zstd integer form, which this writer does not produce; narrow the series range",
+                          a == 0 ? "series ids" : a == 1 ? "row counts" : "last times", at);
+                return OG_E_UNSUPPORTED;
+            }
+            const uint32_t sz = (uint32_t)(out.size() - pos - 4);
+            for (int i = 0; i < 4; i++) out[pos + i] = (uint8_t)(sz >> (24 - 8 * i));
+        }
+    }
+    const uint64_t idtime_size = out.size() - idtime_begin;
+    const uint64_t trailer_off = meta_off + out.size();
+    w.i64(16); w.i64((int64_t)(meta_off - 16)); w.i64((int64_t)index_size); w.i64((int64_t)mi_size); w.i64((int64_t)bloom.size()); w.i64((int64_t)idtime_size);
+    w.i64((int64_t)ids.size()); w.u64(ids.front()); w.u64(ids.back()); w.i64(file_tmin); w.i64(file_tmax); w.i64((int64_t)items.size());
+    w.u64(bloom_m); w.u64(bloom_k);
+    /* ExtraData: time-store flag 1, compress flag 0, no chunk-meta header; its real length (10) in the upper half of the flags */
+    w.u16(8);
+    { const uint64_t flags = 1ull | (10ull << 32); for (int i = 0; i < 8; i++) w.u8((uint32_t)(flags >> (8 * i)) & 0xff); }
+    w.u16(0);
+    const size_t nl = strlen(in.measurement);
+    w.u16((uint32_t)nl); w.bytes(in.measurement, nl);
+    w.i64((int64_t)trailer_off);
+    return OG_OK;
+}

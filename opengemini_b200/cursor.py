@@ -222,6 +222,27 @@ class Shard:
             pass
 
 
+def write_tssp(shard, measurement, series=None, timing=None):
+    """og_shard_write_tssp: the bytes of one TSSP file holding `shard` (any open Shard: from a description or file, synthesised,
+    merged, or a downsample result reopened with Downsampled.open()).  series: (begin, end) half-open range of the shard's series,
+    None = all.  timing: a dict that receives the milliseconds of the call's phases."""
+    d = L.TsspWriteDesc(measurement.encode() if isinstance(measurement, str) else measurement, *((0, 0) if series is None else series), 0)
+    h = C.c_void_p()
+    L.check(L.lib().og_shard_write_tssp(shard.h, C.byref(d), C.byref(h)), "og_shard_write_tssp")
+    try:
+        n = C.c_uint64()
+        L.check(L.lib().og_tssp_image_size(h, C.byref(n)), "og_tssp_image_size")
+        out = np.empty(n.value, np.uint8)
+        L.check(L.lib().og_tssp_image_export(h, out.ctypes.data), "og_tssp_image_export")
+        if timing is not None:
+            ms = (C.c_double * 4)()
+            L.check(L.lib().og_tssp_image_timing(h, ms), "og_tssp_image_timing")
+            timing.update(preagg=ms[0], layout_gather_crc=ms[1], metadata_d2h=ms[2], host_assembly=ms[3])
+    finally:
+        L.lib().og_tssp_image_free(h)
+    return out.tobytes()
+
+
 class Downsampled:
     """Result of Shard.downsample: a shard description whose pages live in device memory (owned by this handle)."""
 
