@@ -48,14 +48,6 @@ static int map_dev_err(int code) {
     }
 }
 
-template <class T> static int dalloc(T **p, size_t n) {
-    *p = nullptr;
-    if (n == 0) n = 1;
-    cudaError_t e = dev_malloc((void **)p, n * sizeof(T));
-    if (e != cudaSuccess) { set_error("cudaMalloc(%zu bytes) failed: %s", n * sizeof(T), cudaGetErrorString(e)); return e == cudaErrorMemoryAllocation ? OG_E_NOMEM : OG_E_CUDA; }
-    return OG_OK;
-}
-
 static DirP make_dir(const og_shard *s) {
     DirP d;
     d.data = s->d_data; d.page_off = s->d_page_off; d.page_len = s->d_page_len; d.seg_series = s->d_seg_series;
@@ -70,42 +62,40 @@ int shard_finalize(og_shard *s, bool scan_snappy) {
     s->il.resize(s->n_columns); /* sized once here: queries only read/lock individual entries later */
     if ((rc = dalloc(&s->d_seg_series, s->n_segments))) return rc;
     if ((rc = dalloc(&s->d_seg_rows, s->n_segments))) return rc;
+    Scratch tmp;
     int32_t *d_types; unsigned long long *d_tot; uint32_t *d_max; int *d_err;
-    if ((rc = dalloc(&d_types, s->n_columns))) return rc;
-    if ((rc = dalloc(&d_tot, 3))) return rc;
-    if ((rc = dalloc(&d_max, 1))) return rc;
-    if ((rc = dalloc(&d_err, 2))) return rc;
+    if ((rc = tmp.get(&d_types, s->n_columns)) || (rc = tmp.get(&d_tot, 3)) || (rc = tmp.get(&d_max, 1)) || (rc = tmp.get(&d_err, 2))) return rc;
     CU(cudaMemcpy(d_types, s->col_types.data(), s->n_columns * sizeof(int32_t), cudaMemcpyHostToDevice));
     CU(cudaMemset(d_tot, 0, 24)); CU(cudaMemset(d_max, 0, 4)); CU(cudaMemset(d_err, 0, 8));
     if (s->n_series) k_fill_seg_series<<<s->n_series, 128>>>(s->d_series_seg_begin, s->n_series, s->d_seg_series);
     if (s->n_segments && scan_snappy) { /* Snappy pages -> raw pages appended behind the data (snappy_load.cuh) */
         const size_t n_pages = (size_t)(s->n_columns + 1) * s->n_segments;
+        Scratch tr;
         uint32_t *tr_size; unsigned long long *d_cnt;
-        if ((rc = dalloc(&tr_size, n_pages))) return rc;
-        if ((rc = dalloc(&d_cnt, 3))) { dev_free(tr_size); return rc; }
-        struct Free2 { void *a, *b; ~Free2() { dev_free(a); dev_free(b); } } f2{tr_size, d_cnt};
+        if ((rc = tr.get(&tr_size, n_pages)) || (rc = tr.get(&d_cnt, 3))) return rc;
         CU(cudaMemset(d_cnt, 0, 24));
         k_snappy_scan<<<(s->n_segments + 127) / 128, 128>>>(make_dir(s), d_types, tr_size, d_cnt);
         unsigned long long cnt[3];
         CU(cudaMemcpy(cnt, d_cnt, 24, cudaMemcpyDeviceToHost));
         if (cnt[0]) {
             if (!s->owns_data) { set_error("shard has %llu Snappy pages: they are transcoded at open, which needs a library-owned copy of the data (do not pass OG_SHARD_DEVICE_DATA)", cnt[0]); return OG_E_UNSUPPORTED; }
-            uint64_t *tr_off; void *tmp = nullptr; size_t tb = 0;
-            if ((rc = dalloc(&tr_off, n_pages))) return rc;
-            struct Free1 { void *a; ~Free1() { dev_free(a); } } f1{tr_off};
+            uint64_t *tr_off; uint8_t *scan_tmp; size_t tb = 0;
+            if ((rc = tr.get(&tr_off, n_pages))) return rc;
             CU(cub::DeviceScan::ExclusiveSum(nullptr, tb, tr_size, tr_off, (int)n_pages));
-            CU(dev_malloc((void **)&tmp, tb ? tb : 1));
-            struct Free3 { void *a; ~Free3() { dev_free(a); } } f3{tmp};
-            CU(cub::DeviceScan::ExclusiveSum(tmp, tb, tr_size, tr_off, (int)n_pages));
+            if ((rc = tr.get(&scan_tmp, tb))) return rc;
+            CU(cub::DeviceScan::ExclusiveSum(scan_tmp, tb, tr_size, tr_off, (int)n_pages));
             const uint64_t new_base = (s->data_len + 15) & ~15ull, new_len = new_base + cnt[2];
+            /* the shard takes the new buffer at once; the loaded pages stay readable until `tr` releases them */
+            const DirP loaded = make_dir(s);
             uint8_t *nd;
             if ((rc = dalloc(&nd, (size_t)new_len + 1024))) return rc;
-            CU(cudaMemcpy(nd, s->d_data, s->data_len, cudaMemcpyDeviceToDevice));
+            tr.bufs.push_back(s->d_data); s->d_data = nd;
+            CU(cudaMemcpy(nd, loaded.data, s->data_len, cudaMemcpyDeviceToDevice));
             CU(cudaMemset(nd + s->data_len, 0, new_len + 1024 - s->data_len));
-            k_snappy_transcode<<<(unsigned)((n_pages + 127) / 128), 128>>>(make_dir(s), tr_size, tr_off, nd, new_base, s->d_page_off, s->d_page_len, d_err);
+            k_snappy_transcode<<<(unsigned)((n_pages + 127) / 128), 128>>>(loaded, tr_size, tr_off, nd, new_base, s->d_page_off, s->d_page_len, d_err);
             CU(cudaGetLastError());
             CU(cudaDeviceSynchronize());
-            dev_free(s->d_data); s->d_data = nd; s->data_len = new_len;
+            s->data_len = new_len;
             s->snappy_pages = cnt[0]; s->snappy_bytes_in = cnt[1]; s->snappy_bytes_out = cnt[2];
         }
     }
@@ -115,13 +105,36 @@ int shard_finalize(og_shard *s, bool scan_snappy) {
     CU(cudaMemcpy(tot, d_tot, 24, cudaMemcpyDeviceToHost));
     CU(cudaMemcpy(err, d_err, 8, cudaMemcpyDeviceToHost));
     CU(cudaMemcpy(&mx, d_max, 4, cudaMemcpyDeviceToHost));
-    dev_free(d_types); dev_free(d_tot); dev_free(d_max); dev_free(d_err);
     if (err[0]) {
         set_error("segment %d: %s page (device validation code %d)", err[1], err[0] == D_UNSUPPORTED ? "unsupported codec in" : err[0] == D_TYPE ? "type mismatch in" : "corrupt", err[0]);
         return map_dev_err(err[0]);
     }
     s->n_rows = tot[0]; s->page_bytes = tot[1] - s->snappy_bytes_out + s->snappy_bytes_in; /* algorithmic bytes = the pages as stored */
     s->max_seg_rows = mx; s->irregular_time_pages = tot[2];
+    return OG_OK;
+}
+
+/* the six directory arrays of a shard whose n_series, n_segments and n_columns are set */
+int alloc_dir(og_shard *s) {
+    const size_t nseg = s->n_segments, n_pages = ((size_t)s->n_columns + 1) * nseg;
+    int rc;
+    if ((rc = dalloc(&s->d_series_seg_begin, (size_t)s->n_series + 1)) || (rc = dalloc(&s->d_tmin, nseg)) || (rc = dalloc(&s->d_tmax, nseg)) ||
+        (rc = dalloc(&s->d_page_off, n_pages)) || (rc = dalloc(&s->d_page_len, n_pages)) || (rc = dalloc(&s->d_sids, (size_t)s->n_series)))
+        return rc;
+    return OG_OK;
+}
+
+/* ... allocated and filled from host arrays of those sizes (page_off / page_len column-major, time column last) */
+int upload_dir(og_shard *s, const uint32_t *series_seg_begin, const int64_t *seg_tmin, const int64_t *seg_tmax, const uint64_t *page_off,
+               const uint32_t *page_len, const uint64_t *sids) {
+    int rc = alloc_dir(s); if (rc) return rc;
+    const size_t nseg = s->n_segments, n_pages = ((size_t)s->n_columns + 1) * nseg;
+    CU(cudaMemcpy(s->d_series_seg_begin, series_seg_begin, ((size_t)s->n_series + 1) * 4, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(s->d_tmin, seg_tmin, nseg * 8, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(s->d_tmax, seg_tmax, nseg * 8, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(s->d_page_off, page_off, n_pages * 8, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(s->d_page_len, page_len, n_pages * 4, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(s->d_sids, sids, (size_t)s->n_series * 8, cudaMemcpyHostToDevice));
     return OG_OK;
 }
 
@@ -188,19 +201,7 @@ int ensure_device() {
 static int need_device() { return ogpu::ensure_device(); }
 extern "C" {
 
-OG_API void og_shard_close(og_shard *s) {
-    if (!s) return;
-    if (s->owns_data && s->d_data) dev_free(s->d_data);
-    dev_free(s->d_series_seg_begin); dev_free(s->d_seg_series); dev_free(s->d_seg_rows); dev_free(s->d_tmin); dev_free(s->d_tmax);
-    dev_free(s->d_page_off); dev_free(s->d_page_len); dev_free(s->d_sids);
-    if (s->h_seg_buf) cudaFreeHost(s->h_seg_buf);
-    if (s->d_seg_buf) dev_free(s->d_seg_buf);
-    for (auto &c : s->il) {
-        dev_free(c.words); dev_free(c.grp_off); dev_free(c.grp_rows); dev_free(c.grp_col); dev_free(c.lane_seg); dev_free(c.lane_rows); dev_free(c.lane_win);
-        dev_free(c.lane_series); dev_free(c.lane_t0); dev_free(c.lane_dt); dev_free(c.gen_list);
-    }
-    delete s;
-}
+OG_API void og_shard_close(og_shard *s) { delete s; }
 
 } // extern "C"
 namespace ogpu {
@@ -234,7 +235,7 @@ OG_API int og_shard_open(const og_shard_desc *d, og_shard **out) {
     *out = nullptr;
     int rc = need_device(); if (rc) return rc;
     if ((rc = check_desc(d))) return rc;
-    og_shard *s = new og_shard;
+    std::unique_ptr<og_shard> s(new og_shard);
     s->device = g_device; s->n_series = d->n_series; s->n_segments = d->n_segments; s->n_columns = d->n_columns;
     s->data_len = d->data_len;
     for (uint32_t c = 0; c < d->n_columns; c++) {
@@ -253,25 +254,15 @@ OG_API int og_shard_open(const og_shard_desc *d, og_shard **out) {
     s->tmin = INT64_MAX; s->tmax = INT64_MIN;
     if (d->n_series)
         for (uint32_t g = d->series_seg_begin[0]; g < d->series_seg_begin[d->n_series]; g++) { s->tmin = std::min(s->tmin, d->seg_tmin[g]); s->tmax = std::max(s->tmax, d->seg_tmax[g]); }
-#define TRY(x) do { rc = (x); if (rc) { og_shard_close(s); return rc; } } while (0)
-#define TRYCU(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { rc = cuda_fail(e_, #x, __FILE__, __LINE__); og_shard_close(s); return rc; } } while (0)
     if (d->flags & OG_SHARD_DEVICE_DATA) { s->d_data = (uint8_t *)d->data; s->owns_data = false; }
     else {
-        TRY(dalloc(&s->d_data, d->data_len + 1024)); /* tail padding: word-wise unaligned loads and the interleave repack read past the last page */
-        TRYCU(cudaMemcpy(s->d_data, d->data, d->data_len, cudaMemcpyHostToDevice));
-        TRYCU(cudaMemset(s->d_data + d->data_len, 0, 1024));
+        if ((rc = dalloc(&s->d_data, d->data_len + 1024))) return rc; /* tail padding: word-wise unaligned loads and the interleave repack read past the last page */
+        CU(cudaMemcpy(s->d_data, d->data, d->data_len, cudaMemcpyHostToDevice));
+        CU(cudaMemset(s->d_data + d->data_len, 0, 1024));
     }
-    TRY(dalloc(&s->d_series_seg_begin, (size_t)d->n_series + 1));
-    TRY(dalloc(&s->d_tmin, nseg)); TRY(dalloc(&s->d_tmax, nseg));
-    TRY(dalloc(&s->d_page_off, ncol1 * nseg)); TRY(dalloc(&s->d_page_len, ncol1 * nseg)); TRY(dalloc(&s->d_sids, (size_t)d->n_series));
-    TRYCU(cudaMemcpy(s->d_series_seg_begin, d->series_seg_begin, ((size_t)d->n_series + 1) * 4, cudaMemcpyHostToDevice));
-    TRYCU(cudaMemcpy(s->d_tmin, d->seg_tmin, nseg * 8, cudaMemcpyHostToDevice));
-    TRYCU(cudaMemcpy(s->d_tmax, d->seg_tmax, nseg * 8, cudaMemcpyHostToDevice));
-    TRYCU(cudaMemcpy(s->d_page_off, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
-    TRYCU(cudaMemcpy(s->d_page_len, len.data(), len.size() * 4, cudaMemcpyHostToDevice));
-    TRYCU(cudaMemcpy(s->d_sids, d->sids, (size_t)d->n_series * 8, cudaMemcpyHostToDevice));
-    TRY(shard_finalize(s, true));
-    *out = s;
+    if ((rc = upload_dir(s.get(), d->series_seg_begin, d->seg_tmin, d->seg_tmax, off.data(), len.data(), d->sids))) return rc;
+    if ((rc = shard_finalize(s.get(), true))) return rc;
+    *out = s.release();
     return OG_OK;
 }
 
@@ -338,21 +329,19 @@ static bool window_clamped(int64_t interval, int64_t offset, int64_t t) {
 
 } /* extern "C" */
 namespace { void free_plan(void *plan); }
-extern "C" {
-void og_query_free_merge_state(void *p);
-OG_API void og_query_destroy(og_query *q) {
-    if (!q) return;
-    if (q->merge_state) og_query_free_merge_state(q->merge_state);
-    free_plan(q->plan);
-    for (void *p : q->scratch) dev_free(p);
-    for (int c = 0; c < OG_MAX_CALLS; c++) { dev_free(q->dense[c].val); dev_free(q->dense[c].ok); dev_free(q->dense[c].tim); }
-    dev_free(q->d_group_of_series);
-    if (q->ev0) cudaEventDestroy(q->ev0);
-    if (q->ev1) cudaEventDestroy(q->ev1);
-    for (cudaEvent_t e : q->main_ev) cudaEventDestroy(e);
-    if (q->stream) cudaStreamDestroy(q->stream);
-    delete q;
+extern "C" void og_query_free_merge_state(void *p);
+/* callers may still have work enqueued on the stream (og_dense_view.stream) that reads the dense record: wait for it */
+og_query::~og_query() {
+    if (stream) cudaStreamSynchronize(stream);
+    og_query_free_merge_state(merge_state);
+    free_plan(plan);
+    if (ev0) cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+    for (cudaEvent_t e : main_ev) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
 }
+extern "C" {
+OG_API void og_query_destroy(og_query *q) { delete q; }
 
 OG_API int og_query_create(og_shard *s, const og_query_desc *d_in, og_query **out) {
     if (!s || !d_in || !out) { set_error("null argument"); return OG_E_INVAL; }
@@ -369,7 +358,7 @@ OG_API int og_query_create(og_shard *s, const og_query_desc *d_in, og_query **ou
     if (d->n_calls == 0 || d->n_calls > OG_MAX_CALLS) { set_error("n_calls must be 1..%d", OG_MAX_CALLS); return OG_E_INVAL; }
     if (d->n_filter > OG_MAX_FILTER) { set_error("filter too long (max %d items)", OG_MAX_FILTER); return OG_E_INVAL; }
     if (d->interval < 0 || d->tmin > d->tmax) { set_error("bad interval or time range"); return OG_E_INVAL; }
-    og_query *q = new og_query;
+    std::unique_ptr<og_query> q(new og_query);
     q->sh = s; q->desc = *d;
     q->calls.assign(d->calls, d->calls + d->n_calls);
     if (d->n_filter) q->filter.assign(d->filter, d->filter + d->n_filter);
@@ -385,12 +374,12 @@ OG_API int og_query_create(og_shard *s, const og_query_desc *d_in, og_query **ou
     };
     for (uint32_t i = 0; i < d->n_calls; i++) {
         const og_call &c = d->calls[i];
-        if (c.column < 0 || (uint32_t)c.column >= s->n_columns || c.func < OG_AGG_COUNT || c.func > OG_AGG_LAST) { set_error("call %u: bad column or function", i); delete q; return OG_E_INVAL; }
+        if (c.column < 0 || (uint32_t)c.column >= s->n_columns || c.func < OG_AGG_COUNT || c.func > OG_AGG_LAST) { set_error("call %u: bad column or function", i); return OG_E_INVAL; }
         int type = s->col_types[c.column];
-        if (type == OG_TYPE_STRING && c.func != OG_AGG_COUNT) { set_error("call %u: only count() is pushed down for string columns (their values are never decoded on the GPU path)", i); delete q; return OG_E_UNSUPPORTED; }
-        if (c.func == OG_AGG_SUM && type == OG_TYPE_BOOL) { set_error("sum() over a boolean column (unsupported sum iterator type, series_call_processor.go:140)"); delete q; return OG_E_INVAL; }
+        if (type == OG_TYPE_STRING && c.func != OG_AGG_COUNT) { set_error("call %u: only count() is pushed down for string columns (their values are never decoded on the GPU path)", i); return OG_E_UNSUPPORTED; }
+        if (c.func == OG_AGG_SUM && type == OG_TYPE_BOOL) { set_error("sum() over a boolean column (unsupported sum iterator type, series_call_processor.go:140)"); return OG_E_INVAL; }
         int sl = slot_of(c.column);
-        if (sl < 0) { set_error("too many distinct columns"); delete q; return OG_E_INVAL; }
+        if (sl < 0) { set_error("too many distinct columns"); return OG_E_INVAL; }
         p.calls[i].func = c.func; p.calls[i].col_slot = sl; p.calls[i].type = type;
         p.calls[i].out_type = c.func == OG_AGG_COUNT ? OG_TYPE_INT : type;
     }
@@ -401,18 +390,18 @@ OG_API int og_query_create(og_shard *s, const og_query_desc *d_in, og_query **ou
         FilterP &fp = p.filter[i];
         fp.kind = f.kind;
         if (f.kind == OG_F_TERM) {
-            if (f.column < 0 || (uint32_t)f.column >= s->n_columns || f.op < OG_OP_LT || f.op > OG_OP_NEQ) { set_error("filter item %u: bad column or op", i); delete q; return OG_E_INVAL; }
-            if (s->col_types[f.column] == OG_TYPE_STRING) { set_error("filter item %u: WHERE on a string column is not pushed down", i); delete q; return OG_E_UNSUPPORTED; }
+            if (f.column < 0 || (uint32_t)f.column >= s->n_columns || f.op < OG_OP_LT || f.op > OG_OP_NEQ) { set_error("filter item %u: bad column or op", i); return OG_E_INVAL; }
+            if (s->col_types[f.column] == OG_TYPE_STRING) { set_error("filter item %u: WHERE on a string column is not pushed down", i); return OG_E_UNSUPPORTED; }
             int sl = slot_of(f.column);
-            if (sl < 0) { set_error("too many distinct columns"); delete q; return OG_E_INVAL; }
+            if (sl < 0) { set_error("too many distinct columns"); return OG_E_INVAL; }
             fp.col_slot = sl; fp.op = f.op; fp.type = s->col_types[f.column]; fp.const_is_float = f.const_is_float; fp.fval = f.fval; fp.ival = f.ival;
             sp++;
         } else if (f.kind == OG_F_AND || f.kind == OG_F_OR) {
-            if (sp < 2) { set_error("filter RPN underflow at item %u", i); delete q; return OG_E_INVAL; }
+            if (sp < 2) { set_error("filter RPN underflow at item %u", i); return OG_E_INVAL; }
             sp--;
-        } else { set_error("filter item %u: bad kind", i); delete q; return OG_E_INVAL; }
+        } else { set_error("filter item %u: bad kind", i); return OG_E_INVAL; }
     }
-    if (d->n_filter && sp != 1) { set_error("filter RPN does not reduce to one value"); delete q; return OG_E_INVAL; }
+    if (d->n_filter && sp != 1) { set_error("filter RPN does not reduce to one value"); return OG_E_INVAL; }
     p.n_filter = d->n_filter;
     /* bucket geometry: TimeWindowsInit (agg_tagset_cursor.go:1012-1027) over the query range (updateQueryTime :448-463) */
     /* FileInfo.{Min,Max}Time is the file range intersected with the query range (fileLoopCursor.updateQueryTime :448-463),
@@ -421,7 +410,7 @@ OG_API int og_query_create(og_shard *s, const og_query_desc *d_in, og_query **ou
     bool overlap = gmin <= gmax;
     if (!overlap) gmin = gmax = d->tmin; /* no overlap: one empty window */
     if (d->flags & OG_Q_QUERY_GRID) { /* one grid for every shard of a cross-shard query */
-        if (d_in->tmin <= MIN_TIME || d_in->tmax >= MAX_TIME) { set_error("OG_Q_QUERY_GRID needs a bounded time range"); delete q; return OG_E_INVAL; }
+        if (d_in->tmin <= MIN_TIME || d_in->tmax >= MAX_TIME) { set_error("OG_Q_QUERY_GRID needs a bounded time range"); return OG_E_INVAL; }
         gmin = d->tmin; gmax = d->tmax; overlap = true;
     }
     int64_t s0, e0, s1, e1;
@@ -429,28 +418,28 @@ OG_API int og_query_create(og_shard *s, const og_query_desc *d_in, og_query **ou
     else {
         /* (a range without rows keeps its one empty window, clamped or not: nothing is placed in it) */
         if (overlap && (window_clamped(d->interval, d->offset, gmin) || window_clamped(d->interval, d->offset, gmax))) {
-            set_error("the first or last window of the range is clamped at the int64 time limits"); delete q; return OG_E_UNSUPPORTED;
+            set_error("the first or last window of the range is clamped at the int64 time limits"); return OG_E_UNSUPPORTED;
         }
         window_of(d->interval, d->offset, d->tmin, d->tmax, gmin, &s0, &e0);
         window_of(d->interval, d->offset, d->tmin, d->tmax, gmax + 1, &s1, &e1);
     }
     p.tmin = d->tmin; p.tmax = d->tmax; p.start = s0; p.interval = e0 - s0;
-    if (p.interval <= 0) { set_error("degenerate window"); delete q; return OG_E_INVAL; }
+    if (p.interval <= 0) { set_error("degenerate window"); return OG_E_INVAL; }
     uint64_t nb = d->interval ? (uint64_t)(e1 - s0) / (uint64_t)p.interval : 1;
-    if (nb == 0 || nb > 0x7fffffffull) { set_error("query range yields %llu buckets", (unsigned long long)nb); delete q; return OG_E_INVAL; }
+    if (nb == 0 || nb > 0x7fffffffull) { set_error("query range yields %llu buckets", (unsigned long long)nb); return OG_E_INVAL; }
     p.n_buckets = (uint32_t)nb;
     /* groups */
     q->n_groups = d->group_mode == OG_GROUP_ALL ? 1 : d->group_mode == OG_GROUP_PER_SERIES ? s->n_series : d->n_groups;
     if (d->group_mode == OG_GROUP_MAP) {
-        if (!d->series_group || d->n_groups == 0) { set_error("OG_GROUP_MAP needs series_group and n_groups"); delete q; return OG_E_INVAL; }
+        if (!d->series_group || d->n_groups == 0) { set_error("OG_GROUP_MAP needs series_group and n_groups"); return OG_E_INVAL; }
         q->series_group.assign(d->series_group, d->series_group + s->n_series);
-        for (uint32_t g : q->series_group) if (g >= d->n_groups) { set_error("series_group entry out of range"); delete q; return OG_E_INVAL; }
-    } else if (d->group_mode != OG_GROUP_ALL && d->group_mode != OG_GROUP_PER_SERIES) { set_error("bad group_mode"); delete q; return OG_E_INVAL; }
+        for (uint32_t g : q->series_group) if (g >= d->n_groups) { set_error("series_group entry out of range"); return OG_E_INVAL; }
+    } else if (d->group_mode != OG_GROUP_ALL && d->group_mode != OG_GROUP_PER_SERIES) { set_error("bad group_mode"); return OG_E_INVAL; }
     if (q->n_groups == 0) q->n_groups = 1;
     cudaError_t e = cudaStreamCreateWithFlags(&q->stream, cudaStreamNonBlocking);
-    if (e != cudaSuccess) { delete q; return cuda_fail(e, "cudaStreamCreate", __FILE__, __LINE__); }
+    if (e != cudaSuccess) return cuda_fail(e, "cudaStreamCreate", __FILE__, __LINE__);
     cudaEventCreate(&q->ev0); cudaEventCreate(&q->ev1);
-    *out = q;
+    *out = q.release();
     return OG_OK;
 }
 
@@ -471,7 +460,6 @@ struct Plan { /* built once per query, reused by every og_query_run */
     const og_shard::IlCol *ic;
 };
 void free_plan(void *plan) { delete (Plan *)plan; }
-template <class T> int salloc(og_query *q, T **p, size_t n) { int rc = dalloc(p, n); if (rc == OG_OK) q->scratch.push_back(*p); return rc; }
 
 template <int NC> void launch_fused(const DirP &d, const QueryP &p, const ChunkP &ch, const uint32_t *list, uint32_t n, cudaStream_t st) {
     if (n) k_fused_segment<NC><<<(n + 127) / 128, 128, 0, st>>>(d, p, ch, list, n);
@@ -544,8 +532,6 @@ void launch_multi(const QueryP &p, const DirP &d, const ChunkP &ch, uint32_t nse
     }
 }
 
-struct TmpBufs { std::vector<void *> v; ~TmpBufs() { for (void *p : v) dev_free(p); } template <class T> int get(T **p, size_t n) { int rc = dalloc(p, n); if (rc == OG_OK) v.push_back(*p); return rc; } };
-
 /* Build (once per shard and column) the lane-interleaved, length-binned stream copy that k_fused_il reads (il_build.cuh).
  * Returns OG_OK with state 1 (ready), -1 (nothing eligible) or -2 (not enough device memory: the general fused kernel
  * serves the column instead; visible in og_stats.il_state). */
@@ -567,7 +553,7 @@ int ensure_il(og_shard *s, int col, cudaStream_t st) {
     int rc;
     struct Ev { cudaEvent_t e = nullptr; Ev() { cudaEventCreate(&e); } ~Ev() { if (e) cudaEventDestroy(e); } } ev0, ev1;
     cudaEventRecord(ev0.e, st);
-    TmpBufs tmp;
+    Scratch tmp(st); /* k_il_scan and the sort may still run on st when a check below returns */
     IlScanOut so{};
     uint32_t *seg_words; uint64_t *keys2; uint32_t *vals2;
     if ((rc = tmp.get(&so.seg_win, nseg)) || (rc = tmp.get(&so.n_packed, 1)) ||
@@ -664,9 +650,9 @@ int build_plan(og_query *q) {
     size_t cells_dense = (size_t)q->n_groups * p.n_buckets;
     for (uint32_t c = 0; c < p.n_calls; c++) { /* dense accumulators (the result) */
         bool sel = p.calls[c].func >= OG_AGG_MIN && !(p.multi && p.calls[c].func <= OG_AGG_MAX);
-        if ((rc = dalloc(&q->dense[c].val, cells_dense))) return rc;
-        if ((rc = dalloc(&q->dense[c].ok, cells_dense))) return rc;
-        if (sel && (rc = dalloc(&q->dense[c].tim, cells_dense))) return rc;
+        if ((rc = q->bufs.get(&q->dense[c].val, cells_dense))) return rc;
+        if ((rc = q->bufs.get(&q->dense[c].ok, cells_dense))) return rc;
+        if (sel && (rc = q->bufs.get(&q->dense[c].tim, cells_dense))) return rc;
     }
     /* group CSR: series sorted by (group, series) */
     std::vector<uint32_t> grp_begin(q->n_groups + 1, 0), grp_series(s->n_series);
@@ -680,9 +666,9 @@ int build_plan(og_query *q) {
         std::iota(grp_series.begin(), grp_series.end(), 0u);
     } else { grp_begin[1] = s->n_series; std::iota(grp_series.begin(), grp_series.end(), 0u); }
     uint32_t *d_grp_begin, *d_grp_series;
-    if ((rc = salloc(q, &d_grp_begin, grp_begin.size()))) return rc;
-    if ((rc = salloc(q, &d_grp_series, grp_series.size()))) return rc;
-    if ((rc = salloc(q, &q->d_err, 16))) return rc;
+    if ((rc = q->bufs.get(&d_grp_begin, grp_begin.size()))) return rc;
+    if ((rc = q->bufs.get(&d_grp_series, grp_series.size()))) return rc;
+    if ((rc = q->bufs.get(&q->d_err, 16))) return rc;
     CU(cudaMemcpyAsync(d_grp_begin, grp_begin.data(), grp_begin.size() * 4, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(d_grp_series, grp_series.data(), grp_series.size() * 4, cudaMemcpyHostToDevice, st));
     CU(cudaStreamSynchronize(st)); /* the host vectors die with this frame */
@@ -744,14 +730,14 @@ int build_plan(og_query *q) {
     size_t chunk_cells = (size_t)std::min(q->chunk_series, s->n_series) * p.n_buckets;
     for (uint32_t c = 0; c < p.n_calls; c++) {
         bool sel = p.calls[c].func >= OG_AGG_MIN;
-        if ((rc = salloc(q, &ch.cells[c].val, chunk_cells))) return rc;
-        if ((rc = salloc(q, &ch.cells[c].ok, chunk_cells))) return rc;
-        if (sel && (rc = salloc(q, &ch.cells[c].tim, chunk_cells))) return rc;
-        if ((rc = salloc(q, &ch.edges[c].val, 2 * (size_t)max_chunk_segs))) return rc;
-        if ((rc = salloc(q, &ch.edges[c].ok, 2 * (size_t)max_chunk_segs))) return rc;
-        if (sel && (rc = salloc(q, &ch.edges[c].tim, 2 * (size_t)max_chunk_segs))) return rc;
+        if ((rc = q->bufs.get(&ch.cells[c].val, chunk_cells))) return rc;
+        if ((rc = q->bufs.get(&ch.cells[c].ok, chunk_cells))) return rc;
+        if (sel && (rc = q->bufs.get(&ch.cells[c].tim, chunk_cells))) return rc;
+        if ((rc = q->bufs.get(&ch.edges[c].val, 2 * (size_t)max_chunk_segs))) return rc;
+        if ((rc = q->bufs.get(&ch.edges[c].ok, 2 * (size_t)max_chunk_segs))) return rc;
+        if (sel && (rc = q->bufs.get(&ch.edges[c].tim, 2 * (size_t)max_chunk_segs))) return rc;
     }
-    if ((rc = salloc(q, &ch.edge_bucket, 2 * (size_t)max_chunk_segs))) return rc;
+    if ((rc = q->bufs.get(&ch.edge_bucket, 2 * (size_t)max_chunk_segs))) return rc;
     pl->blockmerge = !pl->fold && q->desc.group_mode == OG_GROUP_ALL && !(q->desc.flags & OG_Q_STRICT_ORDER) &&
                      (s->n_series > 2 * OG_MERGE_SB || getenv("OGPU_FORCE_BLOCKMERGE") /* test hook */);
     if (pl->blockmerge) { /* block partials of the two-stage merge live in the folded cell matrix: one column per block of series */
@@ -760,9 +746,9 @@ int build_plan(og_query *q) {
         const size_t n = (size_t)p.n_buckets * ch.gc_cols;
         for (uint32_t c = 0; c < p.n_calls; c++) {
             bool sel = p.calls[c].func >= OG_AGG_MIN;
-            if ((rc = salloc(q, &ch.gcells[c].val, n))) return rc;
-            if ((rc = salloc(q, &ch.gcells[c].ok, n))) return rc;
-            if (sel && (rc = salloc(q, &ch.gcells[c].tim, n))) return rc;
+            if ((rc = q->bufs.get(&ch.gcells[c].val, n))) return rc;
+            if ((rc = q->bufs.get(&ch.gcells[c].ok, n))) return rc;
+            if (sel && (rc = q->bufs.get(&ch.gcells[c].tim, n))) return rc;
         }
     }
     if (pl->fold) { /* folded cell matrix: lane-group columns, their tail-window columns, then three columns per block of 32 consecutive
@@ -772,9 +758,9 @@ int build_plan(og_query *q) {
         const size_t n = (size_t)p.n_buckets * ch.gc_cols;
         for (uint32_t c = 0; c < p.n_calls; c++) {
             bool sel = p.calls[c].func >= OG_AGG_MIN;
-            if ((rc = salloc(q, &ch.gcells[c].val, n))) return rc;
-            if ((rc = salloc(q, &ch.gcells[c].ok, n))) return rc;
-            if (sel && (rc = salloc(q, &ch.gcells[c].tim, n))) return rc;
+            if ((rc = q->bufs.get(&ch.gcells[c].val, n))) return rc;
+            if ((rc = q->bufs.get(&ch.gcells[c].ok, n))) return rc;
+            if (sel && (rc = q->bufs.get(&ch.gcells[c].tim, n))) return rc;
         }
     }
     if (pl->fast) {
@@ -801,11 +787,11 @@ int build_plan(og_query *q) {
         q->tile_segs = std::max<uint32_t>(32, q->tile_segs & ~31u);
         tp.S = q->tile_segs;
         for (uint32_t k = 0; k < p.n_cols; k++) {
-            if ((rc = salloc(q, &tp.vals[k], (size_t)q->tile_segs * tp.R))) return rc;
-            if ((rc = salloc(q, &tp.okb[k], (size_t)q->tile_segs * tp.R))) return rc;
+            if ((rc = q->bufs.get(&tp.vals[k], (size_t)q->tile_segs * tp.R))) return rc;
+            if ((rc = q->bufs.get(&tp.okb[k], (size_t)q->tile_segs * tp.R))) return rc;
         }
-        if ((rc = salloc(q, &tp.times, (size_t)q->tile_segs * tp.R))) return rc;
-        if ((rc = salloc(q, &tp.keep, (size_t)q->tile_segs * tp.R))) return rc;
+        if ((rc = q->bufs.get(&tp.times, (size_t)q->tile_segs * tp.R))) return rc;
+        if ((rc = q->bufs.get(&tp.keep, (size_t)q->tile_segs * tp.R))) return rc;
     }
     q->planned = true;
     return OG_OK;
@@ -983,10 +969,11 @@ OG_API int og_query_stats(const og_query *q, og_stats *out) {
     og_query *mq = const_cast<og_query *>(q);
     if (q->ran && q->stats.page_bytes == 0) {
         CU(cudaSetDevice(q->sh->device));
-        unsigned long long *d_o; int rc = dalloc(&d_o, 3); if (rc) return rc;
+        Scratch tmp;
+        unsigned long long *d_o; int rc = tmp.get(&d_o, 3); if (rc) return rc;
         cudaMemset(d_o, 0, 24);
         if (q->sh->n_segments) k_sum_page_bytes<<<(q->sh->n_segments + 255) / 256, 256>>>(make_dir(q->sh), q->qp, q->qp.tmin, q->qp.tmax, d_o);
-        unsigned long long h[3]; CU(cudaMemcpy(h, d_o, 24, cudaMemcpyDeviceToHost)); dev_free(d_o);
+        unsigned long long h[3]; CU(cudaMemcpy(h, d_o, 24, cudaMemcpyDeviceToHost));
         mq->stats.page_bytes = h[0]; mq->stats.rows_decoded = h[1]; mq->stats.segments_scanned = h[2];
     }
     *out = q->stats;
@@ -1191,11 +1178,12 @@ static int decode_segment_impl(og_shard *s, uint32_t segment, uint32_t flags, og
     size_t ncol1 = (size_t)s->n_columns + 1;
     size_t val_stride = (size_t)R * 8, bm_stride = (((size_t)R + 7) / 8 + 7) & ~(size_t)7;
     size_t need = ncol1 * (val_stride + bm_stride + 16);
-    if (s->d_seg_buf_bytes < need) {
-        if (s->d_seg_buf) dev_free(s->d_seg_buf);
+    if (s->d_seg_buf_bytes < need || s->h_seg_buf_bytes < need) { /* a failed allocation leaves a buffer null with size 0 */
+        dev_free(s->d_seg_buf); s->d_seg_buf = nullptr; s->d_seg_buf_bytes = 0;
         if (s->h_seg_buf) cudaFreeHost(s->h_seg_buf);
-        CU(dev_malloc((void **)&s->d_seg_buf, need)); CU(cudaMallocHost(&s->h_seg_buf, need));
-        s->d_seg_buf_bytes = s->h_seg_buf_bytes = need;
+        s->h_seg_buf = nullptr; s->h_seg_buf_bytes = 0;
+        CU(dev_malloc(&s->d_seg_buf, need)); s->d_seg_buf_bytes = need;
+        CU(cudaMallocHost(&s->h_seg_buf, need)); s->h_seg_buf_bytes = need;
     }
     uint8_t *dv = (uint8_t *)s->d_seg_buf, *dbm = dv + ncol1 * val_stride;
     uint32_t *drows = (uint32_t *)(dbm + ncol1 * bm_stride);

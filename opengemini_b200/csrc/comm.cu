@@ -132,7 +132,8 @@ struct og_merge_state { /* per (query, communicator): buffers + the captured gra
     MergeP mp{};
     cudaGraphExec_t graph = nullptr;
     bool geometry_checked = false;
-    void *bufs[4] = {nullptr, nullptr, nullptr, nullptr};
+    Scratch bufs; /* the packed buffers of mp */
+    ~og_merge_state() { if (graph) cudaGraphExecDestroy(graph); }
 };
 
 extern "C" {
@@ -179,23 +180,17 @@ OG_API int og_comm_info(const og_comm *c, int *rank, int *world, int *nccl_versi
 OG_API int og_comm_allreduce_f64(og_comm *c, double *vals, int n, int op_max) {
     if (!c || !vals || n <= 0 || n > 64) return OG_E_INVAL;
     CU(cudaSetDevice(c->device));
-    double *d; CU(dev_malloc((void **)&d, (size_t)n * 8));
+    Scratch tmp;
+    double *d; int rc = tmp.get(&d, (size_t)n); if (rc) return rc;
     CU(cudaMemcpy(d, vals, (size_t)n * 8, cudaMemcpyHostToDevice));
     ncclResult_t r = g_nccl.AllReduce(d, d, (size_t)n, ncclFloat64, op_max ? ncclMax : ncclSum, c->comm, nullptr);
     cudaError_t e = cudaMemcpy(vals, d, (size_t)n * 8, cudaMemcpyDeviceToHost);
-    dev_free(d);
     if (r != ncclSuccess) { set_error("ncclAllReduce failed: %s", g_nccl.GetErrorString(r)); return OG_E_CUDA; }
     if (e != cudaSuccess) return cuda_fail(e, "allreduce copy", __FILE__, __LINE__);
     return OG_OK;
 }
 
-static void merge_state_free(og_merge_state *ms) {
-    if (!ms) return;
-    if (ms->graph) cudaGraphExecDestroy(ms->graph);
-    for (void *p : ms->bufs) dev_free(p);
-    delete ms;
-}
-void og_query_free_merge_state(void *p) { merge_state_free((og_merge_state *)p); }
+void og_query_free_merge_state(void *p) { delete (og_merge_state *)p; }
 
 static int enqueue_merge(og_query *q, og_merge_state *ms, cudaStream_t st) {
     const MergeP &m = ms->mp;
@@ -221,10 +216,10 @@ OG_API int og_query_allreduce(og_query *q, og_comm *c) {
     const QueryP &p = q->qp;
     cudaStream_t st = q->stream;
     og_merge_state *ms = (og_merge_state *)q->merge_state;
-    if (ms && ms->comm != c) { merge_state_free(ms); ms = nullptr; q->merge_state = nullptr; }
-    if (!ms) {
-        ms = new og_merge_state; ms->comm = c; q->merge_state = ms;
-        MergeP &m = ms->mp;
+    if (ms && ms->comm != c) { delete ms; ms = nullptr; q->merge_state = nullptr; }
+    if (!ms) { /* the query keeps it once its buffers are allocated */
+        std::unique_ptr<og_merge_state> nm(new og_merge_state); nm->comm = c;
+        MergeP &m = nm->mp;
         m.n_cols = p.n_calls; m.world = (uint32_t)c->world; m.cells = (uint64_t)q->n_groups * p.n_buckets;
         for (uint32_t k = 0; k < p.n_calls; k++) {
             MergeCol &mc = m.cols[k];
@@ -233,12 +228,11 @@ OG_API int og_query_allreduce(og_query *q, og_comm *c) {
             else if (mc.func == OG_AGG_SUM || mc.func == OG_AGG_COUNT) { mc.kind = 1; mc.slot = m.n_i64++; }
             else { mc.kind = 2; mc.slot = m.n_sel++; }
         }
-        if (m.n_f64) { CU(dev_malloc((void **)&ms->bufs[0], (size_t)m.n_f64 * m.cells * 8)); m.f64 = (double *)ms->bufs[0]; }
-        if (m.n_f64 + m.n_i64) { CU(dev_malloc((void **)&ms->bufs[1], (size_t)(2 * m.n_i64 + m.n_f64) * m.cells * 8)); m.i64 = (int64_t *)ms->bufs[1]; }
-        if (m.n_sel) {
-            CU(dev_malloc((void **)&ms->bufs[2], (size_t)m.n_sel * 3 * m.cells * 8)); m.sel_send = (uint64_t *)ms->bufs[2];
-            CU(dev_malloc((void **)&ms->bufs[3], (size_t)m.world * m.n_sel * 3 * m.cells * 8)); m.sel_recv = (uint64_t *)ms->bufs[3];
-        }
+        int rc;
+        if (m.n_f64 && (rc = nm->bufs.get(&m.f64, (size_t)m.n_f64 * m.cells))) return rc;
+        if (m.n_f64 + m.n_i64 && (rc = nm->bufs.get(&m.i64, (size_t)(2 * m.n_i64 + m.n_f64) * m.cells))) return rc;
+        if (m.n_sel && ((rc = nm->bufs.get(&m.sel_send, (size_t)m.n_sel * 3 * m.cells)) || (rc = nm->bufs.get(&m.sel_recv, (size_t)m.world * m.n_sel * 3 * m.cells)))) return rc;
+        q->merge_state = ms = nm.release();
     }
     if (!ms->geometry_checked) { /* every rank must hold the same grid and the same calls: compare a fingerprint through the communicator */
         double fp[8] = {(double)p.n_buckets, (double)q->n_groups, (double)p.n_calls, (double)(p.start >> 20), (double)(p.start & 0xfffff), (double)(p.interval >> 20), (double)(p.interval & 0xfffff), 0.0};

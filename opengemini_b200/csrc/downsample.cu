@@ -86,19 +86,6 @@ __global__ void k_ds_seg_times(const int64_t *time, const uint32_t *seg_rows, ui
     tmax[g] = time[(size_t)g * DS_ROWS + seg_rows[g] - 1];
 }
 
-template <class T> int dsalloc(T **p, size_t n) {
-    *p = nullptr;
-    cudaError_t e = dev_malloc((void **)p, (n ? n : 1) * sizeof(T));
-    if (e != cudaSuccess) { set_error("device allocation of %zu bytes failed: %s", n * sizeof(T), cudaGetErrorString(e)); return e == cudaErrorMemoryAllocation ? OG_E_NOMEM : OG_E_CUDA; }
-    return OG_OK;
-}
-
-struct Frees { /* device buffers released when the call returns */
-    std::vector<void *> p;
-    ~Frees() { for (void *q : p) dev_free(q); }
-    template <class T> int get(T **out, size_t n) { int rc = dsalloc(out, n); if (rc == OG_OK) p.push_back(*out); return rc; }
-};
-
 /* ---- og_downsample_shard: many output columns, each with its own validity ---- */
 
 struct DsxCol {            /* one output column */
@@ -184,18 +171,12 @@ struct og_downsampled {
     std::vector<std::string> names; std::vector<int32_t> types;
     std::vector<og_column_desc> cols;
     double phase_ms[4] = {0, 0, 0, 0}; /* og_downsample_shard: queries, keep + scatter, encode, directory assembly */
+    ~og_downsampled() { dev_free(d_data); }
 };
-
-#define DS_CU(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) { rc = cuda_fail(e__, #call, __FILE__, __LINE__); goto done; } } while (0)
-#define DS_RC(call) do { rc = (call); if (rc != OG_OK) goto done; } while (0)
 
 extern "C" {
 
-OG_API void og_downsampled_free(og_downsampled *d) {
-    if (!d) return;
-    dev_free(d->d_data);
-    delete d;
-}
+OG_API void og_downsampled_free(og_downsampled *d) { delete d; }
 
 OG_API int og_downsample(og_shard *s, uint32_t column, int64_t interval, int64_t tmin, int64_t tmax, og_downsampled **out) {
     if (!s || !out || interval <= 0) { set_error("bad argument (interval must be > 0)"); return OG_E_INVAL; }
@@ -203,9 +184,7 @@ OG_API int og_downsample(og_shard *s, uint32_t column, int64_t interval, int64_t
     static const int funcs[DS_COLS] = {OG_AGG_MIN, OG_AGG_MAX, OG_AGG_SUM, OG_AGG_COUNT, OG_AGG_FIRST, OG_AGG_LAST};
     static const char *fnames[DS_COLS] = {"min", "max", "sum", "count", "first", "last"};
     int rc = OG_OK;
-    og_query *q = nullptr;
-    og_downsampled *r = nullptr;
-    Frees tmp;
+    Scratch tmp;
     og_shard_layout lay;
     if ((rc = og_shard_layout_get(s, &lay))) return rc;
     if (column >= lay.n_columns) { set_error("column %u out of range", column); return OG_E_INVAL; }
@@ -231,86 +210,81 @@ OG_API int og_downsample(og_shard *s, uint32_t column, int64_t interval, int64_t
     DsSrc src; DsDst dst;
     uint64_t total = 0, cells = 0, pos = 0;
 
-    DS_RC(og_query_create(s, &qd, &q));
-    DS_RC(og_query_run(q));
-    DS_RC(og_query_dense(q, &dv));
+    og_query *qr = nullptr;
+    if ((rc = og_query_create(s, &qd, &qr))) return rc;
+    std::unique_ptr<og_query> q(qr);
+    if ((rc = og_query_run(q.get())) || (rc = og_query_dense(q.get(), &dv))) return rc;
     ns = dv.n_groups; nb = dv.n_buckets;
-    r = new og_downsampled;
+    std::unique_ptr<og_downsampled> r(new og_downsampled);
     r->sids = sids;
     r->ssb.assign((size_t)ns + 1, 0);
     r->off.resize(DS_COLS + 1); r->len.resize(DS_COLS + 1); r->types.resize(DS_COLS);
     if (ns == 0 || nb == 0) goto directory;
 
     /* rows per series -> segments per series -> cell offsets */
-    DS_RC(tmp.get(&d_rows_s, ns));
+    if ((rc = tmp.get(&d_rows_s, ns))) return rc;
     k_ds_count<<<ns, DS_THREADS>>>(dv.cols[3].valid, nb, d_rows_s);
     rows_s.resize(ns);
-    DS_CU(cudaMemcpy(rows_s.data(), d_rows_s, (size_t)ns * 4, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(rows_s.data(), d_rows_s, (size_t)ns * 4, cudaMemcpyDeviceToHost));
     cell_base.resize(ns);
     for (uint32_t i = 0; i < ns; i++) {
         const uint32_t segs = (rows_s[i] + DS_ROWS - 1) / DS_ROWS;
         cell_base[i] = (uint64_t)n_seg * DS_ROWS;
         for (uint32_t g = 0; g < segs; g++) seg_rows.push_back(g + 1 < segs ? DS_ROWS : rows_s[i] - g * DS_ROWS);
-        if ((uint64_t)n_seg + segs > 0xfffffff0ull) { set_error("too many output segments"); rc = OG_E_UNSUPPORTED; goto done; }
+        if ((uint64_t)n_seg + segs > 0xfffffff0ull) { set_error("too many output segments"); return OG_E_UNSUPPORTED; }
         n_seg += segs; r->ssb[i + 1] = n_seg; r->rows += rows_s[i];
     }
     if (n_seg == 0) goto directory;
     cells = (uint64_t)n_seg * DS_ROWS;
-    DS_RC(tmp.get(&d_cell_base, ns));
-    DS_RC(tmp.get(&d_seg_rows, n_seg));
-    DS_CU(cudaMemcpy(d_cell_base, cell_base.data(), (size_t)ns * 8, cudaMemcpyHostToDevice));
-    DS_CU(cudaMemcpy(d_seg_rows, seg_rows.data(), (size_t)n_seg * 4, cudaMemcpyHostToDevice));
+    if ((rc = tmp.get(&d_cell_base, ns)) || (rc = tmp.get(&d_seg_rows, n_seg))) return rc;
+    CU(cudaMemcpy(d_cell_base, cell_base.data(), (size_t)ns * 8, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_seg_rows, seg_rows.data(), (size_t)n_seg * 4, cudaMemcpyHostToDevice));
     for (int c = 0; c < DS_COLS; c++) {
-        DS_RC(tmp.get(&dst.val[c], cells));
-        DS_CU(cudaMemset(dst.val[c], 0, cells * 8)); /* cells past the last row of a series' last segment are never read, but keep them defined */
+        if ((rc = tmp.get(&dst.val[c], cells))) return rc;
+        CU(cudaMemset(dst.val[c], 0, cells * 8)); /* cells past the last row of a series' last segment are never read, but keep them defined */
         src.val[c] = (const uint64_t *)dv.cols[c].values;
     }
-    DS_RC(tmp.get(&d_time, cells));
-    DS_CU(cudaMemset(d_time, 0, cells * 8));
+    if ((rc = tmp.get(&d_time, cells))) return rc;
+    CU(cudaMemset(d_time, 0, cells * 8));
     dst.time = d_time;
     k_ds_scatter<<<ns, DS_THREADS>>>(src, dv.cols[3].valid, nb, dv.start, dv.interval, d_cell_base, dst);
-    DS_CU(cudaGetLastError());
+    CU(cudaGetLastError());
 
     /* segment time ranges */
-    DS_RC(tmp.get(&d_tmin, n_seg)); DS_RC(tmp.get(&d_tmax, n_seg));
+    if ((rc = tmp.get(&d_tmin, n_seg)) || (rc = tmp.get(&d_tmax, n_seg))) return rc;
     k_ds_seg_times<<<(n_seg + 255) / 256, 256>>>(d_time, d_seg_rows, n_seg, d_tmin, d_tmax);
     r->tmin.resize(n_seg); r->tmax.resize(n_seg);
-    DS_CU(cudaMemcpy(r->tmin.data(), d_tmin, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
-    DS_CU(cudaMemcpy(r->tmax.data(), d_tmax, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(r->tmin.data(), d_tmin, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(r->tmax.data(), d_tmax, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
 
     /* encode: six value columns, then time */
-    DS_RC(tmp.get(&d_off, n_seg)); DS_RC(tmp.get(&d_len, n_seg));
+    if ((rc = tmp.get(&d_off, n_seg)) || (rc = tmp.get(&d_len, n_seg))) return rc;
     for (int c = 0; c <= DS_COLS; c++) {
         const bool is_time = c == DS_COLS;
         const int32_t typ = is_time ? OG_TYPE_INT : (funcs[c] == OG_AGG_COUNT ? OG_TYPE_INT : ctype);
         const uint64_t cap = (uint64_t)n_seg * 8800; /* a 1000-row page never exceeds 8 B per row + headers */
-        DS_RC(tmp.get(&d_pages[c], cap));
-        DS_RC(og_encode_pages(typ, is_time ? 1 : 0, is_time ? (const void *)d_time : (const void *)dst.val[c], nullptr, d_seg_rows, n_seg, DS_ROWS,
-                              d_pages[c], cap, d_off, d_len, &page_bytes[c]));
+        if ((rc = tmp.get(&d_pages[c], cap))) return rc;
+        if ((rc = og_encode_pages(typ, is_time ? 1 : 0, is_time ? (const void *)d_time : (const void *)dst.val[c], nullptr, d_seg_rows, n_seg, DS_ROWS,
+                                  d_pages[c], cap, d_off, d_len, &page_bytes[c])))
+            return rc;
         r->off[c].resize(n_seg); r->len[c].resize(n_seg);
-        DS_CU(cudaMemcpy(r->off[c].data(), d_off, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
-        DS_CU(cudaMemcpy(r->len[c].data(), d_len, (size_t)n_seg * 4, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(r->off[c].data(), d_off, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(r->len[c].data(), d_len, (size_t)n_seg * 4, cudaMemcpyDeviceToHost));
         for (uint32_t g = 0; g < n_seg; g++) r->off[c][g] += total;
         total += page_bytes[c];
         if (!is_time) r->types[c] = typ;
     }
     /* one buffer: the columns back to back + the slack word-granular readers need behind the last page */
-    {
-        uint8_t *all = nullptr;
-        cudaError_t e = dev_malloc((void **)&all, total + 1024);
-        if (e != cudaSuccess) { rc = cuda_fail(e, "downsample output", __FILE__, __LINE__); goto done; }
-        r->d_data = all; r->data_len = total;
-        for (int c = 0; c <= DS_COLS; c++) { DS_CU(cudaMemcpy(all + pos, d_pages[c], page_bytes[c], cudaMemcpyDeviceToDevice)); pos += page_bytes[c]; }
-        DS_CU(cudaMemset(all + total, 0, 1024));
-    }
+    if ((rc = dalloc(&r->d_data, total + 1024))) return rc;
+    r->data_len = total;
+    for (int c = 0; c <= DS_COLS; c++) { CU(cudaMemcpy(r->d_data + pos, d_pages[c], page_bytes[c], cudaMemcpyDeviceToDevice)); pos += page_bytes[c]; }
+    CU(cudaMemset(r->d_data + total, 0, 1024));
 
 directory:
     if (!r->d_data) { /* nothing survived: an empty shard still has a valid (zero-length) data region */
-        uint8_t *all = nullptr;
-        cudaError_t e = dev_malloc((void **)&all, 1024);
-        if (e != cudaSuccess) { rc = cuda_fail(e, "downsample output", __FILE__, __LINE__); goto done; }
-        cudaMemset(all, 0, 1024);
-        r->d_data = all; r->data_len = 0;
+        if ((rc = dalloc(&r->d_data, 1024))) return rc;
+        cudaMemset(r->d_data, 0, 1024);
+        r->data_len = 0;
         for (int c = 0; c < DS_COLS; c++) r->types[c] = funcs[c] == OG_AGG_COUNT ? OG_TYPE_INT : ctype;
     }
     for (int c = 0; c < DS_COLS; c++) r->names.push_back(std::string(fnames[c]) + "_f" + std::to_string(column));
@@ -318,13 +292,9 @@ directory:
         og_column_desc cd; cd.name = r->names[c].c_str(); cd.type = r->types[c]; cd.page_off = r->off[c].data(); cd.page_len = r->len[c].data();
         r->cols.push_back(cd);
     }
-    DS_CU(cudaDeviceSynchronize());
-    *out = r; r = nullptr;
-
-done:
-    if (q) og_query_destroy(q);
-    if (r) og_downsampled_free(r);
-    return rc;
+    CU(cudaDeviceSynchronize());
+    *out = r.release();
+    return OG_OK;
 }
 
 /* og_downsample_shard: every field column of the shard under the policy's per-type call lists, in one pass.
@@ -388,14 +358,14 @@ OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_down
     const uint32_t n_oc = (uint32_t)oc.size(), ns = s->n_series;
     if (n_oc + 1 > 65535) { set_error("%u output columns (at most 65534)", n_oc); return OG_E_UNSUPPORTED; }
 
-    std::unique_ptr<og_downsampled, void (*)(og_downsampled *)> r(new og_downsampled, og_downsampled_free);
+    std::unique_ptr<og_downsampled> r(new og_downsampled);
     r->sids = s->sids;
     r->ssb.assign((size_t)ns + 1, 0);
     r->off.resize(n_oc + 1); r->len.resize(n_oc + 1);
     for (const OutCol &c : oc) { r->names.push_back(c.name); r->types.push_back(c.type); }
 
     /* 1. one per-series query per source column, all created before any runs (so a refused range costs no device work) */
-    struct Queries { std::vector<og_query *> q; void clear() { for (og_query *x : q) og_query_destroy(x); q.clear(); } ~Queries() { clear(); } } qs;
+    std::vector<std::unique_ptr<og_query>> qs;
     std::vector<og_dense_view> dv(qcalls.size());
     for (const auto &calls : qcalls) {
         og_query_desc qd{};
@@ -404,11 +374,11 @@ OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_down
         og_query *q = nullptr;
         int rc = og_query_create(s, &qd, &q);
         if (rc) return rc;
-        qs.q.push_back(q);
+        qs.emplace_back(q);
     }
-    for (size_t i = 0; i < qs.q.size(); i++) {
-        int rc = og_query_run(qs.q[i]);
-        if (!rc) rc = og_query_dense(qs.q[i], &dv[i]);
+    for (size_t i = 0; i < qs.size(); i++) {
+        int rc = og_query_run(qs[i].get());
+        if (!rc) rc = og_query_dense(qs[i].get(), &dv[i]);
         if (rc) return rc;
         if (dv[i].start != dv[0].start || dv[i].n_buckets != dv[0].n_buckets || dv[i].interval != dv[0].interval || dv[i].n_groups != ns) {
             set_error("the queries of columns %u and 0 lie on different grids", (unsigned)i); return OG_E_STATE;
@@ -416,7 +386,7 @@ OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_down
     }
     r->phase_ms[0] = ms_since(t_start);
     const uint32_t nb = dv.empty() ? 0 : dv[0].n_buckets;
-    Frees tmp;
+    Scratch tmp;
     uint32_t n_seg = 0;
     uint32_t *d_seg_rows = nullptr;
     int64_t *d_time = nullptr;
@@ -502,19 +472,15 @@ OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_down
             r->len[c].assign(len.begin() + (size_t)c * n_seg, len.begin() + (size_t)(c + 1) * n_seg);
             for (uint64_t &o : r->off[c]) o += col_pos[c];
         }
-        uint8_t *all = nullptr;
-        cudaError_t e = dev_malloc((void **)&all, pos + 1024);
-        if (e != cudaSuccess) return cuda_fail(e, "downsample output", __FILE__, __LINE__);
-        r->d_data = all; r->data_len = pos;
-        CU(cudaMemcpy(all, d_pages, pos, cudaMemcpyDeviceToDevice));
-        CU(cudaMemset(all + pos, 0, 1024));
+        if ((rc = dalloc(&r->d_data, pos + 1024))) return rc;
+        r->data_len = pos;
+        CU(cudaMemcpy(r->d_data, d_pages, pos, cudaMemcpyDeviceToDevice));
+        CU(cudaMemset(r->d_data + pos, 0, 1024));
     }
     if (!r->d_data) { /* nothing survived: an empty shard still has a valid (zero-length) data region */
-        uint8_t *all = nullptr;
-        cudaError_t e = dev_malloc((void **)&all, 1024);
-        if (e != cudaSuccess) return cuda_fail(e, "downsample output", __FILE__, __LINE__);
-        r->d_data = all; r->data_len = 0;
-        CU(cudaMemset(all, 0, 1024));
+        if (int rc = dalloc(&r->d_data, 1024)) return rc;
+        r->data_len = 0;
+        CU(cudaMemset(r->d_data, 0, 1024));
     }
     for (uint32_t c = 0; c < n_oc; c++) {
         og_column_desc cd; cd.name = r->names[c].c_str(); cd.type = r->types[c]; cd.page_off = r->off[c].data(); cd.page_len = r->len[c].data();

@@ -25,6 +25,7 @@
 namespace ogpu {
 
 int shard_finalize(og_shard *s, bool scan_snappy); /* api.cu */
+int alloc_dir(og_shard *s);                        /* api.cu */
 int ensure_device();              /* api.cu */
 
 #define PAGE_STRIDE 8704u /* staging bytes per page: worst case 13 + 125 + 1 + 8000 (raw) rounded up, 8-byte aligned */
@@ -418,13 +419,6 @@ __global__ void k_synth_times(og_synth_desc d, uint32_t seg_begin, uint32_t n_se
     tmin[seg] = c[0]; tmax[seg] = c[n - 1];
 }
 
-template <class T> static int dalloc2(T **p, size_t n) {
-    *p = nullptr;
-    cudaError_t e = dev_malloc((void **)p, std::max<size_t>(1, n) * sizeof(T));
-    if (e != cudaSuccess) { set_error("cudaMalloc(%zu bytes) failed: %s", n * sizeof(T), cudaGetErrorString(e)); return e == cudaErrorMemoryAllocation ? OG_E_NOMEM : OG_E_CUDA; }
-    return OG_OK;
-}
-
 } // namespace ogpu
 
 using namespace ogpu;
@@ -440,11 +434,12 @@ int encode_pages(int32_t type, int32_t is_time, const void *d_values, const uint
     if (type != OG_TYPE_INT && type != OG_TYPE_FLOAT && type != OG_TYPE_BOOL) { set_error("unsupported column type %d", type); return OG_E_UNSUPPORTED; }
     if (n_segments == 0) { if (total_bytes_out) *total_bytes_out = 0; return OG_OK; }
     { int rcd = ensure_device(); if (rcd) return rcd; }
+    Scratch tmp;
     uint8_t *staging; uint64_t *dense = nullptr; int *flags; unsigned long long *d_total;
     int rc;
-    if ((rc = dalloc2(&staging, (size_t)n_segments * PAGE_STRIDE))) return rc;
-    if (type == OG_TYPE_INT && d_valid && !is_time && (rc = dalloc2(&dense, (size_t)n_segments * rps))) { dev_free(staging); return rc; }
-    if ((rc = dalloc2(&flags, 1)) || (rc = dalloc2(&d_total, 1))) { dev_free(staging); dev_free(dense); return rc; }
+    if ((rc = tmp.get(&staging, (size_t)n_segments * PAGE_STRIDE))) return rc;
+    if (type == OG_TYPE_INT && d_valid && !is_time && (rc = tmp.get(&dense, (size_t)n_segments * rps))) return rc;
+    if ((rc = tmp.get(&flags, 1)) || (rc = tmp.get(&d_total, 1))) return rc;
     cudaMemset(flags, 0, 4);
     k_encode_pages<<<(n_segments + 63) / 64, 64>>>(type, is_time, (const uint8_t *)d_values, is_time ? nullptr : d_valid, d_rows, n_segments, rps, staging, d_page_len, dense, flags, nan_raw);
     k_scan_lens<<<1, 1024>>>(d_page_len, n_segments, 0, d_page_off, d_total);
@@ -452,7 +447,6 @@ int encode_pages(int32_t type, int32_t is_time, const void *d_values, const uint
     unsigned long long total = 0; int fl = 0;
     cudaError_t e = cudaMemcpy(&total, d_total, 8, cudaMemcpyDeviceToHost);
     if (e == cudaSuccess) e = cudaMemcpy(&fl, flags, 4, cudaMemcpyDeviceToHost);
-    dev_free(staging); dev_free(dense); dev_free(flags); dev_free(d_total);
     if (e != cudaSuccess) return cuda_fail(e, "og_encode_pages", __FILE__, __LINE__);
     if (fl & 2) { set_error("float column contains +Inf and -Inf (or NaN): FloatArrayEncodeAll rejects it (batch_float.go:245)"); return OG_E_INVAL; }
     if (fl & 16) { set_error("output buffer too small (%llu bytes needed)", total); return OG_E_NOMEM; }
@@ -481,7 +475,7 @@ OG_API int og_shard_synth(const og_synth_desc *dd, og_shard **out) {
     uint64_t nseg64 = (uint64_t)d.n_series * sps;
     if (nseg64 > 0xfffffff0ull) { set_error("too many segments"); return OG_E_INVAL; }
     uint32_t nseg = (uint32_t)nseg64;
-    og_shard *s = new og_shard;
+    std::unique_ptr<og_shard> s(new og_shard);
     s->device = dev; s->n_series = d.n_series; s->n_segments = nseg; s->n_columns = d.n_columns;
     for (uint32_t c = 0; c < d.n_columns; c++) { s->col_types.push_back(d.columns[c].type); s->col_names.push_back("f" + std::to_string(c)); }
     s->sids.resize(d.n_series); s->h_series_seg_begin.resize((size_t)d.n_series + 1);
@@ -489,22 +483,19 @@ OG_API int og_shard_synth(const og_synth_desc *dd, og_shard **out) {
     s->h_series_seg_begin[d.n_series] = nseg;
     s->tmin = d.t0; s->tmax = d.t0 + (int64_t)(d.rows_per_series - 1) * d.dt;
     int rc;
-#define STRY(x) do { rc = (x); if (rc) { og_shard_close(s); return rc; } } while (0)
-#define STRYCU(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { rc = cuda_fail(e_, #x, __FILE__, __LINE__); og_shard_close(s); return rc; } } while (0)
     size_t ncol1 = (size_t)d.n_columns + 1;
-    STRY(dalloc2(&s->d_series_seg_begin, (size_t)d.n_series + 1));
-    STRY(dalloc2(&s->d_tmin, nseg)); STRY(dalloc2(&s->d_tmax, nseg));
-    STRY(dalloc2(&s->d_page_off, ncol1 * nseg)); STRY(dalloc2(&s->d_page_len, ncol1 * nseg)); STRY(dalloc2(&s->d_sids, (size_t)d.n_series));
-    STRYCU(cudaMemcpy(s->d_series_seg_begin, s->h_series_seg_begin.data(), ((size_t)d.n_series + 1) * 4, cudaMemcpyHostToDevice));
-    STRYCU(cudaMemcpy(s->d_sids, s->sids.data(), (size_t)d.n_series * 8, cudaMemcpyHostToDevice));
+    if ((rc = alloc_dir(s.get()))) return rc; /* seg_tmin / seg_tmax and the page directory are filled on the device */
+    CU(cudaMemcpy(s->d_series_seg_begin, s->h_series_seg_begin.data(), ((size_t)d.n_series + 1) * 4, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(s->d_sids, s->sids.data(), (size_t)d.n_series * 8, cudaMemcpyHostToDevice));
     /* batch scratch */
     uint32_t batch = std::min<uint32_t>(nseg, 128u * 1024u);
     uint8_t *cells, *okb, *staging; uint32_t *rows_arr, *lens; uint64_t *offs, *dense; int *flags; unsigned long long *d_total;
-    struct Guard { std::vector<void *> p; ~Guard() { for (void *x : p) dev_free(x); } } guard;
-#define GALLOC(ptr, n) do { STRY(dalloc2(&ptr, n)); guard.p.push_back(ptr); } while (0)
-    GALLOC(cells, (size_t)batch * rps * 8); GALLOC(okb, (size_t)batch * rps); GALLOC(staging, (size_t)batch * PAGE_STRIDE);
-    GALLOC(rows_arr, batch); GALLOC(lens, batch); GALLOC(offs, batch); GALLOC(dense, (size_t)batch * rps); GALLOC(flags, 1); GALLOC(d_total, 1);
-    STRYCU(cudaMemset(flags, 0, 4));
+    Scratch tmp;
+    if ((rc = tmp.get(&cells, (size_t)batch * rps * 8)) || (rc = tmp.get(&okb, (size_t)batch * rps)) || (rc = tmp.get(&staging, (size_t)batch * PAGE_STRIDE)) ||
+        (rc = tmp.get(&rows_arr, batch)) || (rc = tmp.get(&lens, batch)) || (rc = tmp.get(&offs, batch)) || (rc = tmp.get(&dense, (size_t)batch * rps)) ||
+        (rc = tmp.get(&flags, 1)) || (rc = tmp.get(&d_total, 1)))
+        return rc;
+    CU(cudaMemset(flags, 0, 4));
     /* pass 0: size estimate from the first batch of every column, then allocate the blob once */
     std::vector<double> avg(ncol1, 0);
     auto run_batch = [&](uint32_t c, uint32_t b0, uint32_t n, uint8_t *blob, uint64_t base, uint64_t cap, unsigned long long *tot) -> int {
@@ -531,30 +522,30 @@ OG_API int og_shard_synth(const og_synth_desc *dd, og_shard **out) {
     uint64_t est = 0;
     for (uint32_t c = 0; c < ncol1; c++) {
         unsigned long long tot = 0;
-        STRY(run_batch(c, 0, batch, nullptr, 0, 0, &tot));
+        if ((rc = run_batch(c, 0, batch, nullptr, 0, 0, &tot))) return rc;
         avg[c] = (double)tot / batch;
         est += (uint64_t)(avg[c] * 1.02 * nseg) + (1u << 20);
     }
     s->data_len = est;
-    STRY(dalloc2(&s->d_data, est + 1024));
+    if ((rc = dalloc(&s->d_data, est + 1024))) return rc;
     s->owns_data = true;
     uint64_t base = 0;
     for (uint32_t c = 0; c < ncol1; c++) {
         for (uint32_t b0 = 0; b0 < nseg; b0 += batch) {
             uint32_t n = std::min(batch, nseg - b0);
             unsigned long long tot = 0;
-            STRY(run_batch(c, b0, n, s->d_data, base, est, &tot));
+            if ((rc = run_batch(c, b0, n, s->d_data, base, est, &tot))) return rc;
             base += tot;
-            if (base > est) { set_error("synthetic blob estimate too small"); og_shard_close(s); return OG_E_NOMEM; }
+            if (base > est) { set_error("synthetic blob estimate too small"); return OG_E_NOMEM; }
         }
     }
     int fl = 0;
-    STRYCU(cudaMemcpy(&fl, flags, 4, cudaMemcpyDeviceToHost));
-    if (fl & 16) { set_error("synthetic blob overflow"); og_shard_close(s); return OG_E_NOMEM; }
-    STRYCU(cudaMemset(s->d_data + base, 0, std::min<uint64_t>(1024, est + 1024 - base)));
+    CU(cudaMemcpy(&fl, flags, 4, cudaMemcpyDeviceToHost));
+    if (fl & 16) { set_error("synthetic blob overflow"); return OG_E_NOMEM; }
+    CU(cudaMemset(s->d_data + base, 0, std::min<uint64_t>(1024, est + 1024 - base)));
     s->data_len = base;
-    STRY(shard_finalize(s, false));
-    *out = s;
+    if ((rc = shard_finalize(s.get(), false))) return rc;
+    *out = s.release();
     return OG_OK;
 }
 

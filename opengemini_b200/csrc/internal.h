@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <memory>
 #include <string>
 #include <mutex>
 #include <vector>
@@ -23,16 +24,40 @@ int ensure_device(); /* bind the calling thread to the library's device (og_init
 
 /* Device memory comes from the device's stream-ordered pool (cudaMallocAsync on the legacy stream) with its release threshold
  * raised at og_init: shards and queries that are opened and closed in a loop get their buffers back from the pool instead of
- * paying cudaMalloc/cudaFree (tens of ms per GB-sized buffer) every time.  Every buffer is released only after the stream that
- * used it has been synchronised (og_query_run / og_shard_open return synchronised), so reuse across streams is ordered. */
+ * paying cudaMalloc/cudaFree (tens of ms per GB-sized buffer) every time.  A buffer is owned by a handle (og_shard, og_query,
+ * og_downsampled, og_tssp_image, og_merge_state: their destructors free it) or by a Scratch for the length of one call.  The
+ * release goes to the legacy stream, which orders it after legacy-stream work; a buffer used on another stream is released
+ * only after that stream has been synchronised (~og_query and a Scratch bound to the stream do it). */
 inline cudaError_t dev_malloc(void **p, size_t bytes) { return cudaMallocAsync(p, bytes ? bytes : 1, (cudaStream_t)0); }
 inline void dev_free(void *p) { if (p) cudaFreeAsync(p, (cudaStream_t)0); }
+template <class... T> void dev_free_all(T *...p) { (dev_free((void *)p), ...); }
 /* free device memory as a budget sees it: what the driver reports plus what the pool holds but does not use */
 cudaError_t dev_mem_info(size_t *free_b, size_t *total_b);
 #define CU(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return ::ogpu::cuda_fail(e__, #call, __FILE__, __LINE__); } while (0)
 
-struct DevBuf { /* RAII-less helper: explicit free */
-    void *p = nullptr; size_t bytes = 0;
+/* n elements of T (at least one byte); OG_E_NOMEM or OG_E_CUDA with the error text set */
+template <class T> int dalloc(T **p, size_t n) {
+    *p = nullptr;
+    if (n == 0) n = 1;
+    cudaError_t e = dev_malloc((void **)p, n * sizeof(T));
+    if (e != cudaSuccess) { set_error("cudaMalloc(%zu bytes) failed: %s", n * sizeof(T), cudaGetErrorString(e)); return e == cudaErrorMemoryAllocation ? OG_E_NOMEM : OG_E_CUDA; }
+    return OG_OK;
+}
+
+/* device buffers freed together when the Scratch goes out of scope; bound to a stream (not the legacy one), it synchronises
+ * that stream first, so no kernel still enqueued there reads a buffer that went back to the pool */
+struct Scratch {
+    cudaStream_t stream = nullptr;
+    std::vector<void *> bufs;
+    Scratch() = default;
+    explicit Scratch(cudaStream_t st) : stream(st) {}
+    Scratch(const Scratch &) = delete;
+    Scratch &operator=(const Scratch &) = delete;
+    ~Scratch() {
+        if (stream && !bufs.empty()) cudaStreamSynchronize(stream);
+        for (void *p : bufs) dev_free(p);
+    }
+    template <class T> int get(T **p, size_t n) { int rc = dalloc(p, n); if (rc == OG_OK) bufs.push_back(*p); return rc; }
 };
 
 } // namespace ogpu
@@ -74,6 +99,14 @@ struct og_shard {
                    uint64_t n_words = 0, n_packed = 0; /* words of the copy; segments stored as packed XOR deltas */ double build_ms = 0; };
     std::vector<IlCol> il; /* [n_columns] */
     std::mutex il_mu;      /* queries of one shard may be planned from different threads: the build is serialised */
+    ~og_shard() {
+        using ogpu::dev_free_all;
+        if (owns_data) dev_free_all(d_data);
+        dev_free_all(d_series_seg_begin, d_seg_series, d_seg_rows, d_tmin, d_tmax, d_page_off, d_page_len, d_sids, d_seg_buf);
+        if (h_seg_buf) cudaFreeHost(h_seg_buf);
+        for (IlCol &c : il)
+            dev_free_all(c.words, c.grp_off, c.grp_rows, c.grp_col, c.lane_seg, c.lane_rows, c.lane_series, c.lane_win, c.lane_t0, c.lane_dt, c.gen_list);
+    }
 };
 
 namespace ogpu {
@@ -110,10 +143,7 @@ struct og_query {
     /* dense result */
     ogpu::Tri dense[OG_MAX_CALLS]{};
     og_dense_col dense_cols[OG_MAX_CALLS]{};
-    /* group membership CSR on device (series sorted by group, stable) */
-    uint32_t *d_group_of_series = nullptr; /* [n_series] */
-    /* scratch */
-    std::vector<void *> scratch;
+    ogpu::Scratch bufs; /* the dense record and the plan's scratch: freed by ~og_query after it has synchronised the stream */
     og_stats stats{};
     /* host staging for og_query_next */
     std::vector<uint64_t> h_val[OG_MAX_CALLS];
@@ -135,4 +165,5 @@ struct og_query {
     void *plan = nullptr; /* ogpu::Plan (agg_kernels.cuh types) */
     std::vector<cudaEvent_t> main_ev; /* event pairs around the dominant decode+reduce kernels */
     void *merge_state = nullptr;      /* og_merge_state of the last og_query_allreduce (comm.cu) */
+    ~og_query(); /* api.cu */
 };

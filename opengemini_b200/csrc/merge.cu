@@ -40,6 +40,8 @@ namespace ogpu {
 
 int shard_finalize(og_shard *s, bool scan_snappy); /* api.cu */
 int check_desc(const og_shard_desc *d);            /* api.cu */
+int upload_dir(og_shard *s, const uint32_t *series_seg_begin, const int64_t *seg_tmin, const int64_t *seg_tmax, const uint64_t *page_off,
+               const uint32_t *page_len, const uint64_t *sids); /* api.cu */
 int encode_pages(int32_t type, int32_t is_time, const void *d_values, const uint8_t *d_valid, const uint32_t *d_rows, uint32_t n_segments,
                  uint32_t rps, uint8_t *d_out, uint64_t out_cap, uint64_t *d_page_off, uint32_t *d_page_len, uint64_t *total_bytes_out,
                  bool nan_raw); /* encode.cu */
@@ -149,15 +151,6 @@ __global__ void k_merge_combine(const int64_t *t, const uint32_t *perm, const ui
     if (slot == MERGE_RPS - 1 || local == cnt - 1) seg_tmax[g] = tt;
 }
 
-template <class T> static int halloc(std::vector<void *> &keep, T **p, size_t n) {
-    *p = nullptr;
-    cudaError_t e = dev_malloc((void **)p, std::max<size_t>(1, n) * sizeof(T));
-    if (e != cudaSuccess) { set_error("cudaMalloc(%zu bytes) failed: %s", n * sizeof(T), cudaGetErrorString(e)); return e == cudaErrorMemoryAllocation ? OG_E_NOMEM : OG_E_CUDA; }
-    keep.push_back(*p);
-    return OG_OK;
-}
-struct Bufs { std::vector<void *> p; ~Bufs() { for (void *x : p) dev_free(x); } };
-
 static SrcDir dir_of(const og_shard *s) {
     SrcDir d;
     d.data = s->d_data; d.page_off = s->d_page_off; d.page_len = s->d_page_len; d.seg_rows = s->d_seg_rows;
@@ -181,7 +174,7 @@ struct NewSegs { /* what one batch produced, on the host */
 
 /* Merge every span on the device, batch by batch.  Fills batches[] and each span's new-segment range. */
 static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const std::vector<uint32_t> &src_file, const std::vector<uint64_t> &sids, std::vector<NewSegs> &batches,
-                       std::vector<void *> &blobs, uint64_t *replaced_out) {
+                       Scratch &blobs, uint64_t *replaced_out) {
     const uint32_t nc = src->n_columns, ncol1 = nc + 1;
     int rc;
     /* scratch per row: decode (8 t + 4 file + 4 span + 9 per column), sort (4 + 4 perm, 8 keys), heads + scan (8), output slots
@@ -197,8 +190,8 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
     }
     std::vector<int64_t> h_zero;
     unsigned long long *d_rep; MergeErr *d_err; int32_t *d_types;
-    Bufs keep;
-    if ((rc = halloc(keep.p, &d_rep, 1)) || (rc = halloc(keep.p, &d_err, 1)) || (rc = halloc(keep.p, &d_types, nc))) return rc;
+    Scratch keep;
+    if ((rc = keep.get(&d_rep, 1)) || (rc = keep.get(&d_err, 1)) || (rc = keep.get(&d_types, nc))) return rc;
     CU(cudaMemset(d_rep, 0, 8)); CU(cudaMemset(d_err, 0, sizeof(MergeErr)));
     CU(cudaMemcpy(d_types, src->col_types.data(), nc * 4, cudaMemcpyHostToDevice));
     std::vector<uint32_t> seg_rows(src->n_segments);
@@ -219,15 +212,15 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
         }
         h_span_row0.push_back(row);
         const uint32_t nsrc = (uint32_t)h_seg.size();
-        Bufs b;
+        Scratch b;
         uint32_t *d_seg, *d_row0, *d_file, *d_span, *d_span_row0, *row_file, *row_span, *perm_in, *perm, *head, *oidx, *out_begin, *seg_base;
         int64_t *times, *times_sorted; uint64_t *cells; uint8_t *ok;
-        if ((rc = halloc(b.p, &d_seg, nsrc)) || (rc = halloc(b.p, &d_row0, nsrc)) || (rc = halloc(b.p, &d_file, nsrc)) || (rc = halloc(b.p, &d_span, nsrc)) ||
-            (rc = halloc(b.p, &d_span_row0, nsp + 1)) || (rc = halloc(b.p, &row_file, R)) || (rc = halloc(b.p, &row_span, R)) ||
-            (rc = halloc(b.p, &perm_in, R)) || (rc = halloc(b.p, &perm, R)) || (rc = halloc(b.p, &head, (size_t)R + 1)) ||
-            (rc = halloc(b.p, &oidx, (size_t)R + 1)) || (rc = halloc(b.p, &out_begin, nsp + 1)) || (rc = halloc(b.p, &seg_base, nsp)) ||
-            (rc = halloc(b.p, &times, R)) || (rc = halloc(b.p, &times_sorted, R)) || (rc = halloc(b.p, &cells, (size_t)nc * R)) ||
-            (rc = halloc(b.p, &ok, (size_t)nc * R)))
+        if ((rc = b.get(&d_seg, nsrc)) || (rc = b.get(&d_row0, nsrc)) || (rc = b.get(&d_file, nsrc)) || (rc = b.get(&d_span, nsrc)) ||
+            (rc = b.get(&d_span_row0, nsp + 1)) || (rc = b.get(&row_file, R)) || (rc = b.get(&row_span, R)) ||
+            (rc = b.get(&perm_in, R)) || (rc = b.get(&perm, R)) || (rc = b.get(&head, (size_t)R + 1)) ||
+            (rc = b.get(&oidx, (size_t)R + 1)) || (rc = b.get(&out_begin, nsp + 1)) || (rc = b.get(&seg_base, nsp)) ||
+            (rc = b.get(&times, R)) || (rc = b.get(&times_sorted, R)) || (rc = b.get(&cells, (size_t)nc * R)) ||
+            (rc = b.get(&ok, (size_t)nc * R)))
             return rc;
         CU(cudaMemcpy(d_seg, h_seg.data(), nsrc * 4ull, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(d_row0, h_row0.data(), nsrc * 4ull, cudaMemcpyHostToDevice));
@@ -239,7 +232,7 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
         { /* rows of a span by time; stable, so equal times keep file order */
             size_t tb = 0; void *tmp = nullptr;
             CU(cub::DeviceSegmentedSort::StableSortPairs(nullptr, tb, times, times_sorted, perm_in, perm, (int)R, (int)nsp, d_span_row0, d_span_row0 + 1));
-            if ((rc = halloc(b.p, (uint8_t **)&tmp, tb))) return rc;
+            if ((rc = b.get((uint8_t **)&tmp, tb))) return rc;
             CU(cub::DeviceSegmentedSort::StableSortPairs(tmp, tb, times, times_sorted, perm_in, perm, (int)R, (int)nsp, d_span_row0, d_span_row0 + 1));
         }
         /* row_span is constant over a span's rows, so it indexes sorted positions as well as decoded ones */
@@ -247,7 +240,7 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
         {
             size_t tb = 0; void *tmp = nullptr;
             CU(cub::DeviceScan::ExclusiveSum(nullptr, tb, head, oidx, (int)R + 1));
-            if ((rc = halloc(b.p, (uint8_t **)&tmp, tb))) return rc;
+            if ((rc = b.get((uint8_t **)&tmp, tb))) return rc;
             CU(cub::DeviceScan::ExclusiveSum(tmp, tb, head, oidx, (int)R + 1));
         }
         k_merge_span_out<<<(nsp + 1 + 127) / 128, 128>>>(d_span_row0, nsp, oidx, out_begin);
@@ -277,11 +270,11 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
         const size_t out_rows = (size_t)NS * MERGE_RPS;
         int64_t *out_t, *d_tmin, *d_tmax; uint8_t *out_ok; uint32_t *d_rows; uint8_t **d_cols;
         std::vector<uint8_t *> h_cols(nc);
-        if ((rc = halloc(b.p, &out_t, out_rows)) || (rc = halloc(b.p, &out_ok, (size_t)nc * out_rows)) || (rc = halloc(b.p, &d_tmin, NS)) ||
-            (rc = halloc(b.p, &d_tmax, NS)) || (rc = halloc(b.p, &d_rows, NS)) || (rc = halloc(b.p, &d_cols, nc)))
+        if ((rc = b.get(&out_t, out_rows)) || (rc = b.get(&out_ok, (size_t)nc * out_rows)) || (rc = b.get(&d_tmin, NS)) ||
+            (rc = b.get(&d_tmax, NS)) || (rc = b.get(&d_rows, NS)) || (rc = b.get(&d_cols, nc)))
             return rc;
         for (uint32_t c = 0; c < nc; c++)
-            if ((rc = halloc(b.p, &h_cols[c], out_rows * (src->col_types[c] == OG_TYPE_BOOL ? 1 : 8)))) return rc;
+            if ((rc = b.get(&h_cols[c], out_rows * (src->col_types[c] == OG_TYPE_BOOL ? 1 : 8)))) return rc;
         CU(cudaMemcpy(d_cols, h_cols.data(), nc * sizeof(uint8_t *), cudaMemcpyHostToDevice));
         CU(cudaMemcpy(seg_base, h_base.data(), nsp * 4ull, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(d_rows, h_rows.data(), NS * 4ull, cudaMemcpyHostToDevice));
@@ -291,7 +284,7 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
         /* encode every column (string columns: no values inside a span, so no page) */
         uint8_t *blob; uint64_t *d_off; uint32_t *d_len;
         const uint64_t cap = (uint64_t)NS * ncol1 * MERGE_PAGE_BOUND;
-        if ((rc = halloc(b.p, &blob, cap)) || (rc = halloc(b.p, &d_off, (size_t)ncol1 * NS)) || (rc = halloc(b.p, &d_len, (size_t)ncol1 * NS))) return rc;
+        if ((rc = b.get(&blob, cap)) || (rc = b.get(&d_off, (size_t)ncol1 * NS)) || (rc = b.get(&d_len, (size_t)ncol1 * NS))) return rc;
         CU(cudaMemset(d_len, 0, (size_t)ncol1 * NS * 4)); CU(cudaMemset(d_off, 0, (size_t)ncol1 * NS * 8));
         uint64_t used = 0;
         ns.off.assign((size_t)ncol1 * NS, 0); ns.len.assign((size_t)ncol1 * NS, 0);
@@ -312,8 +305,7 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
         CU(cudaMemcpy(ns.tmin.data(), d_tmin, NS * 8ull, cudaMemcpyDeviceToHost));
         CU(cudaMemcpy(ns.tmax.data(), d_tmax, NS * 8ull, cudaMemcpyDeviceToHost));
         /* keep only the bytes written: the batch's scratch goes back to the pool before the next batch */
-        CU(dev_malloc((void **)&ns.blob, std::max<uint64_t>(1, used)));
-        blobs.push_back(ns.blob);
+        if ((rc = blobs.get(&ns.blob, used))) return rc;
         CU(cudaMemcpy(ns.blob, blob, used, cudaMemcpyDeviceToDevice));
         ns.bytes = used;
         batches.push_back(std::move(ns));
@@ -439,36 +431,23 @@ OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_
         span_store.push_back(std::move(sp));
     }
     /* ---- upload (one H2D per file), validate + transcode Snappy over the whole file set ---- */
-    og_shard *src = new og_shard;
+    std::unique_ptr<og_shard> src(new og_shard);
     src->device = dev; src->n_series = (uint32_t)ser0[n_files]; src->n_segments = NSRC; src->n_columns = nc;
     src->col_types = types; src->col_names = names; src->data_len = data_len;
     src->h_series_seg_begin = ssb;
     for (uint32_t f = 0; f < n_files; f++) src->sids.insert(src->sids.end(), files[f].sids, files[f].sids + files[f].n_series);
-#define STRY(x) do { rc = (x); if (rc) { og_shard_close(src); return rc; } } while (0)
-#define STRYCU(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { rc = cuda_fail(e_, #x, __FILE__, __LINE__); og_shard_close(src); return rc; } } while (0)
-    {
-        std::vector<void *> k;
-        STRY(halloc(k, &src->d_data, data_len + 1024));
-        STRYCU(cudaMemset(src->d_data, 0, data_len + 1024));
-        for (uint32_t f = 0; f < n_files; f++)
-            if (files[f].data_len) STRYCU(cudaMemcpy(src->d_data + base[f], files[f].data, files[f].data_len, cudaMemcpyHostToDevice));
-        STRY(halloc(k, &src->d_series_seg_begin, ssb.size()));
-        STRY(halloc(k, &src->d_tmin, NSRC)); STRY(halloc(k, &src->d_tmax, NSRC));
-        STRY(halloc(k, &src->d_page_off, off.size())); STRY(halloc(k, &src->d_page_len, len.size())); STRY(halloc(k, &src->d_sids, src->sids.size()));
-    }
-    STRYCU(cudaMemcpy(src->d_series_seg_begin, ssb.data(), ssb.size() * 4, cudaMemcpyHostToDevice));
-    STRYCU(cudaMemcpy(src->d_tmin, tmin.data(), NSRC * 8ull, cudaMemcpyHostToDevice));
-    STRYCU(cudaMemcpy(src->d_tmax, tmax.data(), NSRC * 8ull, cudaMemcpyHostToDevice));
-    STRYCU(cudaMemcpy(src->d_page_off, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
-    STRYCU(cudaMemcpy(src->d_page_len, len.data(), len.size() * 4, cudaMemcpyHostToDevice));
-    STRYCU(cudaMemcpy(src->d_sids, src->sids.data(), src->sids.size() * 8, cudaMemcpyHostToDevice));
-    STRY(shard_finalize(src, true));
+    if ((rc = dalloc(&src->d_data, data_len + 1024))) return rc;
+    CU(cudaMemset(src->d_data, 0, data_len + 1024));
+    for (uint32_t f = 0; f < n_files; f++)
+        if (files[f].data_len) CU(cudaMemcpy(src->d_data + base[f], files[f].data, files[f].data_len, cudaMemcpyHostToDevice));
+    if ((rc = upload_dir(src.get(), ssb.data(), tmin.data(), tmax.data(), off.data(), len.data(), src->sids.data()))) return rc;
+    if ((rc = shard_finalize(src.get(), true))) return rc;
     /* the transcoded directory and the row counts */
-    STRYCU(cudaMemcpy(off.data(), src->d_page_off, off.size() * 8, cudaMemcpyDeviceToHost));
-    STRYCU(cudaMemcpy(len.data(), src->d_page_len, len.size() * 4, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(off.data(), src->d_page_off, off.size() * 8, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(len.data(), src->d_page_len, len.size() * 4, cudaMemcpyDeviceToHost));
     {
         std::vector<uint32_t> rows(NSRC);
-        STRYCU(cudaMemcpy(rows.data(), src->d_seg_rows, NSRC * 4ull, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(rows.data(), src->d_seg_rows, NSRC * 4ull, cudaMemcpyDeviceToHost));
         for (auto &sp : span_store) {
             for (uint32_t g : sp.src) sp.rows += rows[g];
             info.series_merged++;
@@ -478,43 +457,34 @@ OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_
     }
     /* ---- device merge ---- */
     std::vector<NewSegs> batches;
-    std::vector<void *> blobs;
-    struct FreeBlobs { std::vector<void *> &b; ~FreeBlobs() { for (void *p : b) dev_free(p); } } free_blobs{blobs};
+    Scratch blobs; /* the pages of every batch, until they are copied into the output data */
     cudaEvent_t ev0, ev1;
-    STRYCU(cudaEventCreate(&ev0)); STRYCU(cudaEventCreate(&ev1));
+    CU(cudaEventCreate(&ev0)); CU(cudaEventCreate(&ev1));
     struct FreeEv { cudaEvent_t a, b; ~FreeEv() { cudaEventDestroy(a); cudaEventDestroy(b); } } free_ev{ev0, ev1};
-    STRYCU(cudaEventRecord(ev0, 0));
+    CU(cudaEventRecord(ev0, 0));
     {
         std::vector<Span *> sp;
         for (auto &x : span_store) sp.push_back(&x);
         uint64_t replaced = 0;
-        STRY(merge_spans(src, sp, src_file, sids, batches, blobs, &replaced));
+        if ((rc = merge_spans(src.get(), sp, src_file, sids, batches, blobs, &replaced))) return rc;
         info.rows_replaced = replaced;
     }
     /* ---- final data: the file set's bytes, then the new pages of every batch ---- */
     uint64_t new_len = src->data_len;
     for (auto &b : batches) { b.base = (new_len + 15) & ~15ull; new_len = b.base + b.bytes; }
-    og_shard *s = new og_shard;
+    std::unique_ptr<og_shard> s(new og_shard);
     s->device = dev; s->n_series = NSER; s->n_columns = nc; s->col_types = types; s->col_names = names; s->sids = sids;
     if (batches.empty()) { s->d_data = src->d_data; src->d_data = nullptr; s->data_len = src->data_len; }
     else {
-        std::vector<void *> k;
-        rc = halloc(k, &s->d_data, new_len + 1024);
-        if (rc) { delete s; og_shard_close(src); return rc; }
+        if ((rc = dalloc(&s->d_data, new_len + 1024))) return rc;
         s->data_len = new_len;
-        cudaError_t e = cudaMemset(s->d_data, 0, new_len + 1024);
-        if (e == cudaSuccess) e = cudaMemcpy(s->d_data, src->d_data, src->data_len, cudaMemcpyDeviceToDevice);
-        for (auto &b : batches) if (e == cudaSuccess && b.bytes) e = cudaMemcpy(s->d_data + b.base, b.blob, b.bytes, cudaMemcpyDeviceToDevice);
-        if (e != cudaSuccess) { rc = cuda_fail(e, "merge data copy", __FILE__, __LINE__); og_shard_close(s); og_shard_close(src); return rc; }
+        CU(cudaMemset(s->d_data, 0, new_len + 1024));
+        CU(cudaMemcpy(s->d_data, src->d_data, src->data_len, cudaMemcpyDeviceToDevice));
+        for (auto &b : batches) if (b.bytes) CU(cudaMemcpy(s->d_data + b.base, b.blob, b.bytes, cudaMemcpyDeviceToDevice));
     }
-    {
-        cudaError_t e = cudaEventRecord(ev1, 0);
-        if (e != cudaSuccess) { rc = cuda_fail(e, "cudaEventRecord", __FILE__, __LINE__); og_shard_close(s); og_shard_close(src); return rc; }
-    }
+    CU(cudaEventRecord(ev1, 0));
     if (batches.empty()) { s->snappy_pages = src->snappy_pages; s->snappy_bytes_in = src->snappy_bytes_in; s->snappy_bytes_out = src->snappy_bytes_out; }
-    og_shard_close(src);
-#undef STRY
-#undef STRYCU
+    src.reset();
     /* ---- the output directory ---- */
     std::vector<uint32_t> o_ssb(NSER + 1, 0);
     std::vector<uint64_t> o_off; std::vector<uint32_t> o_len; std::vector<int64_t> o_tmin, o_tmax;
@@ -548,29 +518,14 @@ OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_
     s->n_segments = NOUT; s->h_series_seg_begin = o_ssb;
     s->tmin = INT64_MAX; s->tmax = INT64_MIN;
     for (uint32_t i = 0; i < NOUT; i++) { s->tmin = std::min(s->tmin, o_tmin[i]); s->tmax = std::max(s->tmax, o_tmax[i]); }
-#define TRY(x) do { rc = (x); if (rc) { og_shard_close(s); return rc; } } while (0)
-#define TRYCU(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { rc = cuda_fail(e_, #x, __FILE__, __LINE__); og_shard_close(s); return rc; } } while (0)
-    {
-        std::vector<void *> k;
-        TRY(halloc(k, &s->d_series_seg_begin, o_ssb.size()));
-        TRY(halloc(k, &s->d_tmin, NOUT)); TRY(halloc(k, &s->d_tmax, NOUT));
-        TRY(halloc(k, &s->d_page_off, o_off.size())); TRY(halloc(k, &s->d_page_len, o_len.size())); TRY(halloc(k, &s->d_sids, NSER));
-    }
-    TRYCU(cudaMemcpy(s->d_series_seg_begin, o_ssb.data(), o_ssb.size() * 4, cudaMemcpyHostToDevice));
-    TRYCU(cudaMemcpy(s->d_tmin, o_tmin.data(), NOUT * 8ull, cudaMemcpyHostToDevice));
-    TRYCU(cudaMemcpy(s->d_tmax, o_tmax.data(), NOUT * 8ull, cudaMemcpyHostToDevice));
-    TRYCU(cudaMemcpy(s->d_page_off, o_off.data(), o_off.size() * 8, cudaMemcpyHostToDevice));
-    TRYCU(cudaMemcpy(s->d_page_len, o_len.data(), o_len.size() * 4, cudaMemcpyHostToDevice));
-    TRYCU(cudaMemcpy(s->d_sids, sids.data(), (size_t)NSER * 8, cudaMemcpyHostToDevice));
-    TRY(shard_finalize(s, false));
+    if ((rc = upload_dir(s.get(), o_ssb.data(), o_tmin.data(), o_tmax.data(), o_off.data(), o_len.data(), sids.data()))) return rc;
+    if ((rc = shard_finalize(s.get(), false))) return rc;
     float ms = 0;
-    TRYCU(cudaEventElapsedTime(&ms, ev0, ev1));
+    CU(cudaEventElapsedTime(&ms, ev0, ev1));
     info.merge_ms = ms;
     info.rows_after_merge = s->n_rows;
     s->merge = info;
-#undef TRY
-#undef TRYCU
-    *out = s;
+    *out = s.release();
     return OG_OK;
 }
 

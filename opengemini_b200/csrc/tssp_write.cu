@@ -229,18 +229,6 @@ __global__ void k_tssp_crc_fold(WriteP w, const uint64_t *slot_off, const uint32
     p[0] = (uint8_t)(crc >> 24); p[1] = (uint8_t)(crc >> 16); p[2] = (uint8_t)(crc >> 8); p[3] = (uint8_t)crc;
 }
 
-template <class T> int walloc(T **p, size_t n) {
-    *p = nullptr;
-    cudaError_t e = dev_malloc((void **)p, (n ? n : 1) * sizeof(T));
-    if (e != cudaSuccess) { set_error("device allocation of %zu bytes failed: %s", n * sizeof(T), cudaGetErrorString(e)); return e == cudaErrorMemoryAllocation ? OG_E_NOMEM : OG_E_CUDA; }
-    return OG_OK;
-}
-struct Frees { /* device buffers released when the call returns */
-    std::vector<void *> p;
-    ~Frees() { for (void *q : p) dev_free(q); }
-    template <class T> int get(T **out, size_t n) { int rc = walloc(out, n); if (rc == OG_OK) p.push_back(*out); return rc; }
-};
-
 double ms_since(std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
 
 } // namespace
@@ -250,16 +238,12 @@ struct og_tssp_image {
     uint8_t *d_chunks = nullptr; uint64_t chunk_bytes = 0; /* file bytes [16, 16 + chunk_bytes), on the device */
     std::vector<uint8_t> tail;                             /* everything behind the chunks */
     double phase_ms[4] = {0, 0, 0, 0};
+    ~og_tssp_image() { cudaSetDevice(device); dev_free(d_chunks); }
 };
 
 extern "C" {
 
-OG_API void og_tssp_image_free(og_tssp_image *f) {
-    if (!f) return;
-    cudaSetDevice(f->device);
-    dev_free(f->d_chunks);
-    delete f;
-}
+OG_API void og_tssp_image_free(og_tssp_image *f) { delete f; }
 
 OG_API int og_shard_write_tssp(og_shard *s, const og_tssp_write_desc *d, og_tssp_image **out) {
     if (!s || !d || !out) { set_error("null argument"); return OG_E_INVAL; }
@@ -287,9 +271,9 @@ OG_API int og_shard_write_tssp(og_shard *s, const og_tssp_write_desc *d, og_tssp
     const size_t n_cells = (size_t)w.n_series * w.n_cols1, n_pages = (size_t)w.n_cols1 * w.n_seg, n_slots = n_cells + n_pages;
     if (n_slots + 1 > 0x7fffffffull) { set_error("%zu pages and columns in one file; narrow the series range", n_slots); return OG_E_UNSUPPORTED; }
 
-    std::unique_ptr<og_tssp_image, void (*)(og_tssp_image *)> img(new og_tssp_image, og_tssp_image_free);
+    std::unique_ptr<og_tssp_image> img(new og_tssp_image);
     img->device = s->device;
-    Frees fr;
+    Scratch fr;
     int rc;
     int32_t *d_types; PreAggCell *d_cells; uint8_t *d_state; uint64_t *d_slot_len, *d_slot_off, *d_new_off, *d_chunk_off; uint32_t *d_term; int *d_err;
     if ((rc = fr.get(&d_types, s->n_columns)) || (rc = fr.get(&d_cells, n_cells)) || (rc = fr.get(&d_state, n_cells)) ||
@@ -325,7 +309,7 @@ OG_API int og_shard_write_tssp(og_shard *s, const og_tssp_write_desc *d, og_tssp
                   (unsigned long long)img->chunk_bytes, (unsigned long long)FILE_SIZE_LIMIT);
         return OG_E_UNSUPPORTED;
     }
-    if ((rc = walloc(&img->d_chunks, (size_t)img->chunk_bytes))) return rc;
+    if ((rc = dalloc(&img->d_chunks, (size_t)img->chunk_bytes))) return rc;
     static const CrcPow pw = [] { CrcPow t; uint32_t p = 1u << 30; t.p[0] = p; for (int k = 1; k < 32; k++) t.p[k] = p = crc_mul(p, p); return t; }();
     k_tssp_gather<<<(unsigned)((n_pages * 32 + GATHER_THREADS - 1) / GATHER_THREADS), GATHER_THREADS>>>(w, d_slot_off, pw, img->d_chunks, d_new_off, d_term);
     CU(cudaGetLastError());
