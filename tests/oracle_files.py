@@ -319,12 +319,13 @@ def read_files(files, q, flt=None, chunk=CHUNK_SIZE_NUM, seg_rows=1000):
     return out
 
 
-def scan_aggregate_files(files, query, flt=None):
+def scan_aggregate_files(files, query, flt=None, seg_rows=1000):
     """Aggregate the file set as the reference does: read_files, then the CPU oracle's aggregate cursor + tagset merge over one
     ordered shard whose segments are those records.  `query` is the AggQuery whose descriptor (without its WHERE) is scanned;
-    `flt` is the WHERE as (column name, op, const) RPN terms, applied per file."""
+    `flt` is the WHERE as (column name, op, const) RPN terms, applied per file; `seg_rows` is the segment length of the ordered files
+    (each of their segments is one record)."""
     d = query.desc
-    recs = read_files(files, {"tmin": d.tmin, "tmax": d.tmax}, flt, chunk=d.chunk_size if d.chunk_size > 0 else CHUNK_SIZE_NUM)
+    recs = read_files(files, {"tmin": d.tmin, "tmax": d.tmax}, flt, chunk=d.chunk_size if d.chunk_size > 0 else CHUNK_SIZE_NUM, seg_rows=seg_rows)
     names = sorted({n for f, _ in files for s in f.values() for n in s["cols"]})
     types = {n: t for f, _ in files for s in f.values() for n, (t, _v, _k) in s["cols"].items()}
     blob, pos = [], 0
