@@ -421,8 +421,8 @@ typedef struct og_downsample_desc {
     const og_downsample_ops *ops;   /* [n_types] at most one entry per type; a type without an entry drops its fields */
 } og_downsample_desc;
 OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_downsampled **out);
-/* wall-clock milliseconds of og_downsample_shard's phases: [0] the per-column queries, [1] k_dsx_keep + scan + k_dsx_scatter,
- * [2] page encoding, [3] directory assembly and the output copy.  All zero for og_downsample results. */
+/* wall-clock milliseconds of the phases of og_downsample and og_downsample_shard: [0] the per-column queries, [1] k_dsx_keep +
+ * scan + k_dsx_scatter, [2] page encoding, [3] directory assembly and the output copy. */
 OG_API int og_downsampled_timing(const og_downsampled *d, double phase_ms[4]);
 OG_API int og_downsampled_desc(const og_downsampled *d, og_shard_desc *desc, uint64_t *rows /* may be NULL */);
 OG_API int og_downsampled_export(const og_downsampled *d, uint8_t *host_data /* desc->data_len bytes */);

@@ -1,19 +1,17 @@
 /*
- * downsample.cu — og_downsample: the read-aggregate-write pass of a downsample / level compaction behind ONE C-ABI call
- * (configs[4]).  Replaces, for one field column of one shard: engine/record_plan.go:494-830 (FileSequenceAggregator pulls
- * records, newProcessor reduces them per series and window) feeding engine/immutable/stream_downsample.go:454-600 (the
- * downsampled columns go through the ordinary column builders, column_builder.go:151-349, chunkdata_builder.go:65-97).
+ * downsample.cu — the read-aggregate-write pass of a downsample / level compaction behind ONE C-ABI call (configs[4]).
+ * Replaces engine/record_plan.go:494-830 (FileSequenceAggregator pulls records, newProcessor reduces them per series and window)
+ * feeding engine/immutable/stream_downsample.go:454-600 (the downsampled columns go through the ordinary column builders,
+ * column_builder.go:151-349, chunkdata_builder.go:65-97).
  *
- *   1. og_query_run with OG_GROUP_PER_SERIES and the six calls min, max, sum, count, first, last  -> dense [series][window]
- *   2. k_ds_count / k_ds_scatter: windows without rows are dropped (TransIntervalRec2Rec, lib/record/record.go:1298-1365), the
- *      kept windows of a series are packed front to back (stable) and cut into 1000-row segments (lib/util/util.go:72); the row
- *      time is the window start
- *   3. og_encode_pages per output column and for the time column
- *   4. the directory of the new shard (ChunkMeta contents: segment time ranges, page offsets / sizes) is assembled on the host
+ * Two entry points, one pass (downsample_pass):
+ *   og_downsample_shard  every field column of the shard under a per-type call list, <call>_<field> columns sorted by name
+ *   og_downsample        one numeric column with min, max, sum, count, first, last, columns <call>_f<column> in that order
  *
- * Everything heavy stays on the device; the host sees one u32 per series, and two i64 plus seven (offset, size) pairs per
- * output segment.  The page bytes stay in HBM: og_downsampled_desc describes them with OG_SHARD_DEVICE_DATA, so the new shard can
- * be opened and queried in place, or copied out with og_downsampled_export to be written to a file.
+ * Everything heavy stays on the device; the host sees two numbers per series, a null flag per output column, and two i64 plus
+ * one (offset, size) pair per output column per output segment.  The page bytes stay in HBM: og_downsampled_desc describes
+ * them with OG_SHARD_DEVICE_DATA, so the new shard can be opened and queried in place, or copied out with og_downsampled_export
+ * to be written to a file.
  */
 #include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
@@ -34,59 +32,8 @@ using namespace ogpu;
 namespace {
 
 constexpr uint32_t DS_ROWS = 1000; /* rows per segment of the output (lib/util/util.go:72) */
-constexpr int DS_COLS = 6;         /* min, max, sum, count, first, last */
 constexpr int DS_THREADS = 256;
-
-/* rows_out[s] = windows of series s that hold rows */
-__global__ void k_ds_count(const uint8_t *keep, uint32_t nb, uint32_t *rows_out) {
-    typedef cub::BlockReduce<uint32_t, DS_THREADS> Reduce;
-    __shared__ typename Reduce::TempStorage tmp;
-    const uint8_t *k = keep + (size_t)blockIdx.x * nb;
-    uint32_t n = 0;
-    for (uint32_t b = threadIdx.x; b < nb; b += DS_THREADS) n += k[b] != 0;
-    n = Reduce(tmp).Sum(n);
-    if (threadIdx.x == 0) rows_out[blockIdx.x] = n;
-}
-
-struct DsSrc { const uint64_t *val[DS_COLS]; };
-struct DsDst { uint64_t *val[DS_COLS]; int64_t *time; };
-
-/* block per series: kept windows, in time order, to cells [cell_base[s] + rank] of every output column */
-__global__ void k_ds_scatter(DsSrc src, const uint8_t *keep, uint32_t nb, int64_t start, int64_t interval, const uint64_t *cell_base, DsDst dst) {
-    typedef cub::BlockScan<uint32_t, DS_THREADS> Scan;
-    __shared__ typename Scan::TempStorage tmp;
-    __shared__ uint32_t carry;
-    const size_t row0 = (size_t)blockIdx.x * nb;
-    const uint64_t base = cell_base[blockIdx.x];
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (uint32_t b0 = 0; b0 < nb; b0 += DS_THREADS) {
-        const uint32_t b = b0 + threadIdx.x;
-        const uint32_t k = (b < nb && keep[row0 + b]) ? 1u : 0u;
-        uint32_t rank, total;
-        Scan(tmp).ExclusiveSum(k, rank, total);
-        const uint32_t before = carry;
-        if (k) {
-            const uint64_t at = base + before + rank;
-#pragma unroll
-            for (int c = 0; c < DS_COLS; c++) dst.val[c][at] = src.val[c][row0 + b];
-            dst.time[at] = start + (int64_t)b * interval;
-        }
-        __syncthreads(); /* everyone has read carry and is done with tmp */
-        if (threadIdx.x == 0) carry = before + total;
-        __syncthreads();
-    }
-}
-
-/* first / last row time of every output segment */
-__global__ void k_ds_seg_times(const int64_t *time, const uint32_t *seg_rows, uint32_t n_seg, int64_t *tmin, int64_t *tmax) {
-    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= n_seg) return;
-    tmin[g] = time[(size_t)g * DS_ROWS];
-    tmax[g] = time[(size_t)g * DS_ROWS + seg_rows[g] - 1];
-}
-
-/* ---- og_downsample_shard: many output columns, each with its own validity ---- */
+const char *const FNAME[OG_AGG_LAST + 1] = {"", "count", "sum", "min", "max", "first", "last"};
 
 struct DsxCol {            /* one output column */
     const uint64_t *src;   /* dense [series][window] 8-byte cells of the query that computed it */
@@ -114,10 +61,11 @@ __global__ void k_dsx_keep(const uint8_t *const *ok, uint32_t n_ok, uint32_t nb,
 }
 
 /* block per (series, output column); blockIdx.y == n_cols is the time column, which also writes each segment's row count and
- * time range.  Kept windows go, in time order, to rows [seg_base[s] * DS_ROWS + rank] of the column. */
+ * time range.  Kept windows go, in time order, to rows [seg_base[s] * DS_ROWS + rank] of the column; col_nulls[c] is set when
+ * column c has a null cell in a kept window. */
 __global__ void k_dsx_scatter(const DsxCol *cols, uint32_t n_cols, const uint8_t *keep, uint32_t nb, int64_t start, int64_t interval,
                               const uint32_t *rows_s, const uint64_t *seg_base, int64_t *time, uint32_t *seg_rows, int64_t *seg_tmin,
-                              int64_t *seg_tmax) {
+                              int64_t *seg_tmax, uint32_t *col_nulls) {
     typedef cub::BlockScan<uint32_t, DS_THREADS> Scan;
     __shared__ typename Scan::TempStorage tmp;
     __shared__ uint32_t carry;
@@ -151,6 +99,7 @@ __global__ void k_dsx_scatter(const DsxCol *cols, uint32_t n_cols, const uint8_t
                 if (col.bool_cells) ((uint8_t *)col.dst)[at] = v != 0;
                 else ((uint64_t *)col.dst)[at] = v;
                 col.dst_ok[at] = ok;
+                if (!ok) col_nulls[blockIdx.y] = 1;
             }
         }
         __syncthreads(); /* everyone has read carry and is done with tmp */
@@ -159,6 +108,9 @@ __global__ void k_dsx_scatter(const DsxCol *cols, uint32_t n_cols, const uint8_t
         if (carry == n) break; /* block-uniform: the series' last kept window is placed */
     }
 }
+
+/* one output column: the cells of call `call` of query `query` (indices into downsample_pass's call lists) */
+struct OutCol { std::string name; int32_t type; uint32_t query, call; };
 
 } // namespace
 
@@ -170,193 +122,26 @@ struct og_downsampled {
     std::vector<std::vector<uint64_t>> off; std::vector<std::vector<uint32_t>> len; /* [n_columns + 1], time last */
     std::vector<std::string> names; std::vector<int32_t> types;
     std::vector<og_column_desc> cols;
-    double phase_ms[4] = {0, 0, 0, 0}; /* og_downsample_shard: queries, keep + scatter, encode, directory assembly */
+    double phase_ms[4] = {0, 0, 0, 0}; /* queries, keep + scatter, encode, directory assembly */
     ~og_downsampled() { dev_free(d_data); }
 };
 
-extern "C" {
-
-OG_API void og_downsampled_free(og_downsampled *d) { delete d; }
-
-OG_API int og_downsample(og_shard *s, uint32_t column, int64_t interval, int64_t tmin, int64_t tmax, og_downsampled **out) {
-    if (!s || !out || interval <= 0) { set_error("bad argument (interval must be > 0)"); return OG_E_INVAL; }
-    *out = nullptr;
-    static const int funcs[DS_COLS] = {OG_AGG_MIN, OG_AGG_MAX, OG_AGG_SUM, OG_AGG_COUNT, OG_AGG_FIRST, OG_AGG_LAST};
-    static const char *fnames[DS_COLS] = {"min", "max", "sum", "count", "first", "last"};
-    int rc = OG_OK;
-    Scratch tmp;
-    og_shard_layout lay;
-    if ((rc = og_shard_layout_get(s, &lay))) return rc;
-    if (column >= lay.n_columns) { set_error("column %u out of range", column); return OG_E_INVAL; }
-    std::vector<int32_t> col_types(lay.n_columns);
-    std::vector<uint64_t> sids(lay.n_series);
-    if ((rc = og_shard_export(s, nullptr, sids.data(), nullptr, nullptr, nullptr, nullptr, nullptr, col_types.data()))) return rc;
-    const int32_t ctype = col_types[column];
-    if (ctype != OG_TYPE_FLOAT && ctype != OG_TYPE_INT) { set_error("downsample of a column of type %d", ctype); return OG_E_UNSUPPORTED; }
-
-    og_call calls[DS_COLS];
-    for (int c = 0; c < DS_COLS; c++) { calls[c].func = funcs[c]; calls[c].column = (int32_t)column; }
-    og_query_desc qd{};
-    qd.interval = interval; qd.tmin = tmin; qd.tmax = tmax; qd.ascending = 1; qd.n_calls = DS_COLS; qd.calls = calls;
-    qd.group_mode = OG_GROUP_PER_SERIES;
-    og_dense_view dv;
-    uint32_t ns = 0, nb = 0, n_seg = 0;
-    std::vector<uint32_t> rows_s, seg_rows;
-    std::vector<uint64_t> cell_base;
-    uint32_t *d_rows_s = nullptr, *d_seg_rows = nullptr; uint64_t *d_cell_base = nullptr;
-    int64_t *d_time = nullptr, *d_tmin = nullptr, *d_tmax = nullptr;
-    uint8_t *d_pages[DS_COLS + 1]; uint64_t page_bytes[DS_COLS + 1];
-    uint64_t *d_off = nullptr; uint32_t *d_len = nullptr;
-    DsSrc src; DsDst dst;
-    uint64_t total = 0, cells = 0, pos = 0;
-
-    og_query *qr = nullptr;
-    if ((rc = og_query_create(s, &qd, &qr))) return rc;
-    std::unique_ptr<og_query> q(qr);
-    if ((rc = og_query_run(q.get())) || (rc = og_query_dense(q.get(), &dv))) return rc;
-    ns = dv.n_groups; nb = dv.n_buckets;
-    std::unique_ptr<og_downsampled> r(new og_downsampled);
-    r->sids = sids;
-    r->ssb.assign((size_t)ns + 1, 0);
-    r->off.resize(DS_COLS + 1); r->len.resize(DS_COLS + 1); r->types.resize(DS_COLS);
-    if (ns == 0 || nb == 0) goto directory;
-
-    /* rows per series -> segments per series -> cell offsets */
-    if ((rc = tmp.get(&d_rows_s, ns))) return rc;
-    k_ds_count<<<ns, DS_THREADS>>>(dv.cols[3].valid, nb, d_rows_s);
-    rows_s.resize(ns);
-    CU(cudaMemcpy(rows_s.data(), d_rows_s, (size_t)ns * 4, cudaMemcpyDeviceToHost));
-    cell_base.resize(ns);
-    for (uint32_t i = 0; i < ns; i++) {
-        const uint32_t segs = (rows_s[i] + DS_ROWS - 1) / DS_ROWS;
-        cell_base[i] = (uint64_t)n_seg * DS_ROWS;
-        for (uint32_t g = 0; g < segs; g++) seg_rows.push_back(g + 1 < segs ? DS_ROWS : rows_s[i] - g * DS_ROWS);
-        if ((uint64_t)n_seg + segs > 0xfffffff0ull) { set_error("too many output segments"); return OG_E_UNSUPPORTED; }
-        n_seg += segs; r->ssb[i + 1] = n_seg; r->rows += rows_s[i];
-    }
-    if (n_seg == 0) goto directory;
-    cells = (uint64_t)n_seg * DS_ROWS;
-    if ((rc = tmp.get(&d_cell_base, ns)) || (rc = tmp.get(&d_seg_rows, n_seg))) return rc;
-    CU(cudaMemcpy(d_cell_base, cell_base.data(), (size_t)ns * 8, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(d_seg_rows, seg_rows.data(), (size_t)n_seg * 4, cudaMemcpyHostToDevice));
-    for (int c = 0; c < DS_COLS; c++) {
-        if ((rc = tmp.get(&dst.val[c], cells))) return rc;
-        CU(cudaMemset(dst.val[c], 0, cells * 8)); /* cells past the last row of a series' last segment are never read, but keep them defined */
-        src.val[c] = (const uint64_t *)dv.cols[c].values;
-    }
-    if ((rc = tmp.get(&d_time, cells))) return rc;
-    CU(cudaMemset(d_time, 0, cells * 8));
-    dst.time = d_time;
-    k_ds_scatter<<<ns, DS_THREADS>>>(src, dv.cols[3].valid, nb, dv.start, dv.interval, d_cell_base, dst);
-    CU(cudaGetLastError());
-
-    /* segment time ranges */
-    if ((rc = tmp.get(&d_tmin, n_seg)) || (rc = tmp.get(&d_tmax, n_seg))) return rc;
-    k_ds_seg_times<<<(n_seg + 255) / 256, 256>>>(d_time, d_seg_rows, n_seg, d_tmin, d_tmax);
-    r->tmin.resize(n_seg); r->tmax.resize(n_seg);
-    CU(cudaMemcpy(r->tmin.data(), d_tmin, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(r->tmax.data(), d_tmax, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
-
-    /* encode: six value columns, then time */
-    if ((rc = tmp.get(&d_off, n_seg)) || (rc = tmp.get(&d_len, n_seg))) return rc;
-    for (int c = 0; c <= DS_COLS; c++) {
-        const bool is_time = c == DS_COLS;
-        const int32_t typ = is_time ? OG_TYPE_INT : (funcs[c] == OG_AGG_COUNT ? OG_TYPE_INT : ctype);
-        const uint64_t cap = (uint64_t)n_seg * 8800; /* a 1000-row page never exceeds 8 B per row + headers */
-        if ((rc = tmp.get(&d_pages[c], cap))) return rc;
-        if ((rc = og_encode_pages(typ, is_time ? 1 : 0, is_time ? (const void *)d_time : (const void *)dst.val[c], nullptr, d_seg_rows, n_seg, DS_ROWS,
-                                  d_pages[c], cap, d_off, d_len, &page_bytes[c])))
-            return rc;
-        r->off[c].resize(n_seg); r->len[c].resize(n_seg);
-        CU(cudaMemcpy(r->off[c].data(), d_off, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
-        CU(cudaMemcpy(r->len[c].data(), d_len, (size_t)n_seg * 4, cudaMemcpyDeviceToHost));
-        for (uint32_t g = 0; g < n_seg; g++) r->off[c][g] += total;
-        total += page_bytes[c];
-        if (!is_time) r->types[c] = typ;
-    }
-    /* one buffer: the columns back to back + the slack word-granular readers need behind the last page */
-    if ((rc = dalloc(&r->d_data, total + 1024))) return rc;
-    r->data_len = total;
-    for (int c = 0; c <= DS_COLS; c++) { CU(cudaMemcpy(r->d_data + pos, d_pages[c], page_bytes[c], cudaMemcpyDeviceToDevice)); pos += page_bytes[c]; }
-    CU(cudaMemset(r->d_data + total, 0, 1024));
-
-directory:
-    if (!r->d_data) { /* nothing survived: an empty shard still has a valid (zero-length) data region */
-        if ((rc = dalloc(&r->d_data, 1024))) return rc;
-        cudaMemset(r->d_data, 0, 1024);
-        r->data_len = 0;
-        for (int c = 0; c < DS_COLS; c++) r->types[c] = funcs[c] == OG_AGG_COUNT ? OG_TYPE_INT : ctype;
-    }
-    for (int c = 0; c < DS_COLS; c++) r->names.push_back(std::string(fnames[c]) + "_f" + std::to_string(column));
-    for (int c = 0; c < DS_COLS; c++) {
-        og_column_desc cd; cd.name = r->names[c].c_str(); cd.type = r->types[c]; cd.page_off = r->off[c].data(); cd.page_len = r->len[c].data();
-        r->cols.push_back(cd);
-    }
-    CU(cudaDeviceSynchronize());
-    *out = r.release();
-    return OG_OK;
-}
-
-/* og_downsample_shard: every field column of the shard under the policy's per-type call lists, in one pass.
- *   1. one og_query per source column (its type's calls, OG_GROUP_PER_SERIES, the same range and interval): dense records that
- *      stay on the device; all of them lie on one grid
- *   2. k_dsx_keep: a series keeps a window where any of its output cells is non-null; a device scan turns the segments each
- *      series fills into segment offsets.  k_dsx_scatter: every output column's kept cells, and the time column, segment-major
+/* The pass behind both entry points: one og_query per list in `qcalls`, the output columns `oc` taken from their results.
+ *   1. one og_query per call list (OG_GROUP_PER_SERIES, the same range and interval): dense records that stay on the device;
+ *      all of them lie on one grid
+ *   2. k_dsx_keep: a series keeps a window where any of its output cells is non-null (empty windows are dropped,
+ *      TransIntervalRec2Rec, lib/record/record.go:1298-1365); a device scan turns the 1000-row segments each series fills into
+ *      segment offsets.  k_dsx_scatter: every output column's kept cells, and the time column (the window start), segment-major
  *   3. og_encode_pages per output column (with validity: pages of columns that are null in a kept window carry a bitmap) and for
  *      the time column
  *   4. the directory on the host, from per-series row counts and per-segment time ranges, page offsets and lengths */
-OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_downsampled **out) {
+static int downsample_pass(og_shard *s, int64_t interval, int64_t tmin, int64_t tmax, const std::vector<std::vector<og_call>> &qcalls,
+                           const std::vector<OutCol> &oc, og_downsampled **out) {
     using clock = std::chrono::steady_clock;
     auto ms_since = [](clock::time_point t0) { return std::chrono::duration<double, std::milli>(clock::now() - t0).count(); };
-    static const char *fname[OG_AGG_LAST + 1] = {"", "count", "sum", "min", "max", "first", "last"};
-    if (!s || !d || !out) { set_error("null argument"); return OG_E_INVAL; }
-    *out = nullptr;
-    if (d->interval <= 0 || d->tmin > d->tmax) { set_error("bad argument (interval must be > 0 and tmin <= tmax)"); return OG_E_INVAL; }
-    if (d->n_types && !d->ops) { set_error("n_types is %u but ops is NULL", d->n_types); return OG_E_INVAL; }
-
-    /* the policy: at most one call list per type, each call at most once, and only calls the type has a reducer for */
-    const og_downsample_ops *by_type[OG_TYPE_BOOL + 1] = {};
-    for (uint32_t i = 0; i < d->n_types; i++) {
-        const og_downsample_ops &o = d->ops[i];
-        if (o.type != OG_TYPE_INT && o.type != OG_TYPE_FLOAT && o.type != OG_TYPE_STRING && o.type != OG_TYPE_BOOL) { set_error("ops[%u]: unknown field type %d", i, o.type); return OG_E_INVAL; }
-        if (by_type[o.type]) { set_error("ops[%u]: a second call list for field type %d", i, o.type); return OG_E_INVAL; }
-        if (o.n_funcs && !o.funcs) { set_error("ops[%u]: n_funcs is %u but funcs is NULL", i, o.n_funcs); return OG_E_INVAL; }
-        uint32_t seen = 0;
-        for (uint32_t k = 0; k < o.n_funcs; k++) {
-            const int32_t f = o.funcs[k];
-            if (f < OG_AGG_COUNT || f > OG_AGG_LAST) { set_error("ops[%u].funcs[%u]: bad function %d", i, k, f); return OG_E_INVAL; }
-            if (seen & (1u << f)) { set_error("ops[%u]: %s() listed twice", i, fname[f]); return OG_E_INVAL; }
-            seen |= 1u << f;
-            if (o.type == OG_TYPE_BOOL && f == OG_AGG_SUM) { set_error("ops[%u]: sum() over boolean fields (the reference has no boolean sum reducer)", i); return OG_E_INVAL; }
-            if (o.type == OG_TYPE_STRING && f != OG_AGG_COUNT) {
-                set_error("ops[%u]: %s() over string fields is not supported: only count() is, because string values are never decoded on the device", i, fname[f]);
-                return OG_E_UNSUPPORTED;
-            }
-        }
-        by_type[o.type] = &o;
-    }
     CU(cudaSetDevice(s->device));
     const auto t_start = clock::now();
-
-    /* output columns: <call>_<field> for every field whose type has calls, sorted by name (og_shard_desc's schema order) */
-    struct OutCol { std::string name; int32_t type; uint32_t query, call; };
-    std::vector<OutCol> oc;
-    std::vector<std::vector<og_call>> qcalls; /* per source column, in the order of its type's call list */
-    for (uint32_t c = 0; c < s->n_columns; c++) {
-        const int32_t typ = s->col_types[c];
-        const og_downsample_ops *o = typ >= 0 && typ <= OG_TYPE_BOOL ? by_type[typ] : nullptr;
-        if (!o || o->n_funcs == 0) continue; /* a type without calls drops its fields */
-        std::vector<og_call> calls;
-        for (uint32_t k = 0; k < o->n_funcs; k++) {
-            const int32_t f = o->funcs[k];
-            oc.push_back({std::string(fname[f]) + "_" + s->col_names[c], f == OG_AGG_COUNT ? OG_TYPE_INT : typ, (uint32_t)qcalls.size(), k});
-            calls.push_back({f, (int32_t)c});
-        }
-        qcalls.push_back(calls);
-    }
-    std::stable_sort(oc.begin(), oc.end(), [](const OutCol &a, const OutCol &b) { return a.name < b.name; });
     const uint32_t n_oc = (uint32_t)oc.size(), ns = s->n_series;
-    if (n_oc + 1 > 65535) { set_error("%u output columns (at most 65534)", n_oc); return OG_E_UNSUPPORTED; }
 
     std::unique_ptr<og_downsampled> r(new og_downsampled);
     r->sids = s->sids;
@@ -364,12 +149,12 @@ OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_down
     r->off.resize(n_oc + 1); r->len.resize(n_oc + 1);
     for (const OutCol &c : oc) { r->names.push_back(c.name); r->types.push_back(c.type); }
 
-    /* 1. one per-series query per source column, all created before any runs (so a refused range costs no device work) */
+    /* 1. one per-series query per call list, all created before any runs (so a refused range costs no device work) */
     std::vector<std::unique_ptr<og_query>> qs;
     std::vector<og_dense_view> dv(qcalls.size());
     for (const auto &calls : qcalls) {
         og_query_desc qd{};
-        qd.interval = d->interval; qd.tmin = d->tmin; qd.tmax = d->tmax; qd.ascending = 1;
+        qd.interval = interval; qd.tmin = tmin; qd.tmax = tmax; qd.ascending = 1;
         qd.n_calls = (uint32_t)calls.size(); qd.calls = calls.data(); qd.group_mode = OG_GROUP_PER_SERIES;
         og_query *q = nullptr;
         int rc = og_query_create(s, &qd, &q);
@@ -391,6 +176,7 @@ OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_down
     uint32_t *d_seg_rows = nullptr;
     int64_t *d_time = nullptr;
     std::vector<DsxCol> hcols(n_oc);
+    std::vector<uint32_t> col_nulls(n_oc);
     if (n_oc && ns && nb) {
         /* 2. kept windows, segment offsets, scatter */
         auto t2 = clock::now();
@@ -416,7 +202,7 @@ OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_down
         for (uint32_t i = 0; i < ns; i++) { r->ssb[i + 1] = (uint32_t)base[i + 1]; r->rows += rows_s[i]; }
         if (n_seg) {
             const uint64_t cells = (uint64_t)n_seg * DS_ROWS;
-            int64_t *d_tmin = nullptr, *d_tmax = nullptr; DsxCol *d_cols = nullptr;
+            int64_t *d_tmin = nullptr, *d_tmax = nullptr; DsxCol *d_cols = nullptr; uint32_t *d_nulls = nullptr;
             for (uint32_t c = 0; c < n_oc; c++) {
                 const bool b1 = oc[c].type == OG_TYPE_BOOL;
                 uint8_t *dst = nullptr, *dst_ok = nullptr;
@@ -427,22 +213,25 @@ OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_down
                 hcols[c] = DsxCol{(const uint64_t *)dc.values, dc.valid, dst, dst_ok, b1 ? 1 : 0};
             }
             if ((rc = tmp.get(&d_cols, n_oc)) || (rc = tmp.get(&d_time, cells)) || (rc = tmp.get(&d_seg_rows, n_seg)) ||
-                (rc = tmp.get(&d_tmin, n_seg)) || (rc = tmp.get(&d_tmax, n_seg))) return rc;
+                (rc = tmp.get(&d_tmin, n_seg)) || (rc = tmp.get(&d_tmax, n_seg)) || (rc = tmp.get(&d_nulls, n_oc))) return rc;
             CU(cudaMemcpy(d_cols, hcols.data(), n_oc * sizeof(DsxCol), cudaMemcpyHostToDevice));
             CU(cudaMemset(d_time, 0, cells * 8));
+            CU(cudaMemset(d_nulls, 0, n_oc * 4));
             k_dsx_scatter<<<dim3(ns, n_oc + 1), DS_THREADS>>>(d_cols, n_oc, d_keep, nb, dv[0].start, dv[0].interval, d_rows, d_base, d_time,
-                                                              d_seg_rows, d_tmin, d_tmax);
+                                                              d_seg_rows, d_tmin, d_tmax, d_nulls);
             CU(cudaGetLastError());
             r->tmin.resize(n_seg); r->tmax.resize(n_seg);
             CU(cudaMemcpy(r->tmin.data(), d_tmin, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
             CU(cudaMemcpy(r->tmax.data(), d_tmax, (size_t)n_seg * 8, cudaMemcpyDeviceToHost));
+            CU(cudaMemcpy(col_nulls.data(), d_nulls, n_oc * 4, cudaMemcpyDeviceToHost));
         }
         qs.clear(); /* the dense records have been read */
         r->phase_ms[1] = ms_since(t2);
     }
     auto t4 = clock::now();
     if (n_seg) {
-        /* 3. encode every output column, then time, into one scratch region */
+        /* 3. encode every output column, then time, into one scratch region.  A column without null cells goes without its
+         *    validity bytes: the pages are the same, and the encoder skips a read per row (and, for int, a compacting copy). */
         auto t3 = clock::now();
         const uint64_t cap_col = (uint64_t)n_seg * 8800; /* a 1000-row page never exceeds 8 B per row + headers */
         const uint64_t bound = cap_col * (n_oc + 1);
@@ -456,7 +245,7 @@ OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_down
             uint64_t bytes = 0;
             col_pos[c] = pos;
             rc = og_encode_pages(is_time ? OG_TYPE_INT : oc[c].type, is_time ? 1 : 0, is_time ? (const void *)d_time : hcols[c].dst,
-                                 is_time ? nullptr : hcols[c].dst_ok, d_seg_rows, n_seg, DS_ROWS, d_pages + pos, bound - pos,
+                                 is_time || !col_nulls[c] ? nullptr : hcols[c].dst_ok, d_seg_rows, n_seg, DS_ROWS, d_pages + pos, bound - pos,
                                  d_off + (size_t)c * n_seg, d_len + (size_t)c * n_seg, &bytes);
             if (rc) return rc;
             pos += bytes;
@@ -490,6 +279,75 @@ OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_down
     r->phase_ms[3] = ms_since(t4);
     *out = r.release();
     return OG_OK;
+}
+
+extern "C" {
+
+OG_API void og_downsampled_free(og_downsampled *d) { delete d; }
+
+OG_API int og_downsample(og_shard *s, uint32_t column, int64_t interval, int64_t tmin, int64_t tmax, og_downsampled **out) {
+    if (!s || !out || interval <= 0) { set_error("bad argument (interval must be > 0)"); return OG_E_INVAL; }
+    *out = nullptr;
+    if (column >= s->n_columns) { set_error("column %u out of range", column); return OG_E_INVAL; }
+    const int32_t ctype = s->col_types[column];
+    if (ctype != OG_TYPE_FLOAT && ctype != OG_TYPE_INT) { set_error("downsample of a column of type %d", ctype); return OG_E_UNSUPPORTED; }
+    static const int32_t funcs[] = {OG_AGG_MIN, OG_AGG_MAX, OG_AGG_SUM, OG_AGG_COUNT, OG_AGG_FIRST, OG_AGG_LAST};
+    std::vector<std::vector<og_call>> qcalls(1);
+    std::vector<OutCol> oc;
+    for (uint32_t k = 0; k < 6; k++) {
+        qcalls[0].push_back({funcs[k], (int32_t)column});
+        oc.push_back({std::string(FNAME[funcs[k]]) + "_f" + std::to_string(column), funcs[k] == OG_AGG_COUNT ? OG_TYPE_INT : ctype, 0, k});
+    }
+    return downsample_pass(s, interval, tmin, tmax, qcalls, oc, out);
+}
+
+/* og_downsample_shard: every field column of the shard under the policy's per-type call lists, in one pass */
+OG_API int og_downsample_shard(og_shard *s, const og_downsample_desc *d, og_downsampled **out) {
+    if (!s || !d || !out) { set_error("null argument"); return OG_E_INVAL; }
+    *out = nullptr;
+    if (d->interval <= 0 || d->tmin > d->tmax) { set_error("bad argument (interval must be > 0 and tmin <= tmax)"); return OG_E_INVAL; }
+    if (d->n_types && !d->ops) { set_error("n_types is %u but ops is NULL", d->n_types); return OG_E_INVAL; }
+
+    /* the policy: at most one call list per type, each call at most once, and only calls the type has a reducer for */
+    const og_downsample_ops *by_type[OG_TYPE_BOOL + 1] = {};
+    for (uint32_t i = 0; i < d->n_types; i++) {
+        const og_downsample_ops &o = d->ops[i];
+        if (o.type != OG_TYPE_INT && o.type != OG_TYPE_FLOAT && o.type != OG_TYPE_STRING && o.type != OG_TYPE_BOOL) { set_error("ops[%u]: unknown field type %d", i, o.type); return OG_E_INVAL; }
+        if (by_type[o.type]) { set_error("ops[%u]: a second call list for field type %d", i, o.type); return OG_E_INVAL; }
+        if (o.n_funcs && !o.funcs) { set_error("ops[%u]: n_funcs is %u but funcs is NULL", i, o.n_funcs); return OG_E_INVAL; }
+        uint32_t seen = 0;
+        for (uint32_t k = 0; k < o.n_funcs; k++) {
+            const int32_t f = o.funcs[k];
+            if (f < OG_AGG_COUNT || f > OG_AGG_LAST) { set_error("ops[%u].funcs[%u]: bad function %d", i, k, f); return OG_E_INVAL; }
+            if (seen & (1u << f)) { set_error("ops[%u]: %s() listed twice", i, FNAME[f]); return OG_E_INVAL; }
+            seen |= 1u << f;
+            if (o.type == OG_TYPE_BOOL && f == OG_AGG_SUM) { set_error("ops[%u]: sum() over boolean fields (the reference has no boolean sum reducer)", i); return OG_E_INVAL; }
+            if (o.type == OG_TYPE_STRING && f != OG_AGG_COUNT) {
+                set_error("ops[%u]: %s() over string fields is not supported: only count() is, because string values are never decoded on the device", i, FNAME[f]);
+                return OG_E_UNSUPPORTED;
+            }
+        }
+        by_type[o.type] = &o;
+    }
+
+    /* output columns: <call>_<field> for every field whose type has calls, sorted by name (og_shard_desc's schema order) */
+    std::vector<OutCol> oc;
+    std::vector<std::vector<og_call>> qcalls; /* per source column, in the order of its type's call list */
+    for (uint32_t c = 0; c < s->n_columns; c++) {
+        const int32_t typ = s->col_types[c];
+        const og_downsample_ops *o = typ >= 0 && typ <= OG_TYPE_BOOL ? by_type[typ] : nullptr;
+        if (!o || o->n_funcs == 0) continue; /* a type without calls drops its fields */
+        std::vector<og_call> calls;
+        for (uint32_t k = 0; k < o->n_funcs; k++) {
+            const int32_t f = o->funcs[k];
+            oc.push_back({std::string(FNAME[f]) + "_" + s->col_names[c], f == OG_AGG_COUNT ? OG_TYPE_INT : typ, (uint32_t)qcalls.size(), k});
+            calls.push_back({f, (int32_t)c});
+        }
+        qcalls.push_back(calls);
+    }
+    std::stable_sort(oc.begin(), oc.end(), [](const OutCol &a, const OutCol &b) { return a.name < b.name; });
+    if (oc.size() + 1 > 65535) { set_error("%u output columns (at most 65534)", (unsigned)oc.size()); return OG_E_UNSUPPORTED; }
+    return downsample_pass(s, d->interval, d->tmin, d->tmax, qcalls, oc, out);
 }
 
 OG_API int og_downsampled_timing(const og_downsampled *d, double phase_ms[4]) {

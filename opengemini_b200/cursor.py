@@ -185,7 +185,8 @@ class Shard:
         return out
 
     def downsample(self, column, interval, tmin, tmax):
-        """og_downsample: per-series min/max/sum/count/first/last of `column` per window -> re-encoded pages, in one library call."""
+        """og_downsample: per-series min/max/sum/count/first/last of `column` per window -> re-encoded pages, in one library call
+        (the pass downsample_shard runs, with those six calls on one float or int field)."""
         h = C.c_void_p()
         L.check(L.lib().og_downsample(self.h, column, interval, tmin, tmax, C.byref(h)), "og_downsample")
         return Downsampled(h.value)
@@ -244,7 +245,7 @@ def write_tssp(shard, measurement, series=None, timing=None):
 
 
 class Downsampled:
-    """Result of Shard.downsample: a shard description whose pages live in device memory (owned by this handle)."""
+    """Result of Shard.downsample or Shard.downsample_shard: a shard description whose pages live in device memory (owned by this handle)."""
 
     def __init__(self, h):
         self.h = h
@@ -263,7 +264,7 @@ class Downsampled:
         return out[:self.desc.data_len]
 
     def timing(self):
-        """Milliseconds of og_downsample_shard's phases (zeros for og_downsample results)."""
+        """Milliseconds of the downsample pass's phases."""
         ms = (C.c_double * 4)()
         L.check(L.lib().og_downsampled_timing(self.h, ms), "og_downsampled_timing")
         return dict(queries=ms[0], keep_scatter=ms[1], encode=ms[2], assembly=ms[3])

@@ -251,10 +251,12 @@ def test_segment_cuts_and_ranges_cut_mid_segment(interval):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("typ,dist", [(L.TYPE_FLOAT, L.SYNTH_F_HI), (L.TYPE_INT, L.SYNTH_INT_WALK)])
-def test_agrees_with_og_downsample(typ, dist):
+@pytest.mark.parametrize("typ,dist,nulls", [(L.TYPE_FLOAT, L.SYNTH_F_HI, 0), (L.TYPE_INT, L.SYNTH_INT_WALK, 0), (L.TYPE_FLOAT, L.SYNTH_F_HI, 400)],
+                         ids=["float", "int", "float_nulls"])
+def test_agrees_with_og_downsample(typ, dist, nulls):
+    """The two entry points differ only in column names and order, with nulls too (3-second windows whose rows are all null)."""
     from opengemini_b200 import Shard
-    sh = Shard.synth(5, 4321, [(typ, dist, 0)], t0=T0, dt=SEC, seed=13)
+    sh = Shard.synth(5, 4321, [(typ, dist, nulls)], t0=T0, dt=SEC, seed=13)
     tmin, tmax, ivl = T0 + 5 * SEC, T0 + 4310 * SEC, 3 * SEC
     a = sh.downsample(0, ivl, tmin, tmax)
     b = sh.downsample_shard(ivl, tmin, tmax, {typ: ALL6})
