@@ -260,7 +260,7 @@ OG_API void og_tssp_free(og_tssp *t);
 
 /* ---- shard ---- */
 OG_API int og_shard_open(const og_shard_desc *desc, og_shard **out);
-OG_API void og_shard_close(og_shard *s);
+OG_API void og_shard_close(og_shard *s); /* queries of a closed shard may still be destroyed (og_query_destroy), not run */
 OG_API int og_shard_info(const og_shard *s, uint64_t *n_series, uint64_t *n_segments, uint64_t *n_rows,
                          uint64_t *page_bytes, int64_t *tmin, int64_t *tmax);
 
@@ -295,7 +295,27 @@ typedef struct og_merge_info {
                                         on the legacy stream; includes the host work between batches and the device-to-device copy
                                         of the file set's data region) */
 } og_merge_info;
-OG_API int og_shard_merge_info(const og_shard *s, og_merge_info *out); /* og_shard_open / og_shard_synth shards: n_files = 1, zeros */
+OG_API int og_shard_merge_info(const og_shard *s, og_merge_info *out); /* og_shard_open / og_shard_synth shards: n_files = 1, zeros;
+                                                                         after og_shard_append_files: that call's files and counters */
+
+/* Adds files flushed after the shard was built.  files[] are in file-sequence order, oldest first, every one newer than every
+ * file the shard holds; OG_FILE_OUT_OF_ORDER marks the out-of-order ones.  Afterwards the shard answers every entry point as
+ * og_shard_open_files over its original files followed by these would, with one difference after out-of-order rows: each append
+ * re-encodes the spans its own files touch, where the open re-encodes the hull of all of them, so the rewritten rows can be cut
+ * into different segments.  og_shard_info's n_segments and page_bytes, the directory, and float sums of merged series (rounding)
+ * may then differ from the open's; rows, counts, min / max / first / last and n_rows / tmin / tmax do not.
+ *   The flush rule (engine/mutable/ts_table.go SplitRecordByTime): an appended ordered file's segments of a series start after
+ *   the last time the shard holds for that series; one that does not is OG_E_UNSUPPORTED, naming the sid.
+ *   Refused as og_shard_open_files refuses them, with the same statuses: a column with two types, OG_SHARD_DEVICE_DATA in files[],
+ *   string values inside a re-encoded span, a time repeated within one file inside a span, corrupt pages.  While an og_query
+ *   created on the shard is alive the call is OG_E_STATE (og_query_create on another thread waits while an append runs).
+ *   On every error the shard stays as it was; only its interleaved copies may have been dropped (rebuilt on first use).
+ *   Column and series indices move when a new name or sid sorts into the middle: rebuild series group maps after an append.
+ *   Cost: the new files are copied in, validated and transcoded; spans are merged as at open; then the pages the new directory
+ *   references are copied once, device to device, into a new data region (pages no longer referenced are left behind).  Peak
+ *   device memory: about the live pages twice, plus the new files and the merge scratch.  A shard opened in place
+ *   (OG_SHARD_DEVICE_DATA) gets its own buffer; the caller's buffer is never written. */
+OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files);
 
 /* ---- query (aggregate cursor tree) ---- */
 /* OG_E_UNSUPPORTED when the first or last row in range lies in a window that Window() clamps at the int64 time limits

@@ -126,7 +126,7 @@ EXPORTS = [
     "og_downsample", "og_downsampled_desc", "og_downsampled_export", "og_downsampled_free",
     "og_downsample_shard", "og_downsampled_timing",
     "og_tssp_parse", "og_tssp_desc", "og_tssp_measurement", "og_tssp_time_range", "og_tssp_free",
-    "og_shard_open_files", "og_shard_merge_info",
+    "og_shard_open_files", "og_shard_merge_info", "og_shard_append_files",
     "og_shard_write_tssp", "og_tssp_image_size", "og_tssp_image_export", "og_tssp_image_timing", "og_tssp_image_free",
 ]
 
@@ -157,6 +157,7 @@ def lib():
     L.og_shard_open.argtypes = [C.POINTER(ShardDesc), C.POINTER(C.c_void_p)]
     L.og_shard_open_files.argtypes = [C.POINTER(ShardDesc), u32p, C.c_uint32, C.POINTER(C.c_void_p)]
     L.og_shard_merge_info.argtypes = [C.c_void_p, C.POINTER(MergeInfo)]
+    L.og_shard_append_files.argtypes = [C.c_void_p, C.POINTER(ShardDesc), u32p, C.c_uint32]
     L.og_shard_close.argtypes = [C.c_void_p]
     L.og_shard_close.restype = None
     L.og_shard_info.argtypes = [C.c_void_p, u64p, u64p, u64p, u64p, i64p, i64p]

@@ -333,6 +333,7 @@ extern "C" void og_query_free_merge_state(void *p);
 /* callers may still have work enqueued on the stream (og_dense_view.stream) that reads the dense record: wait for it */
 og_query::~og_query() {
     if (stream) cudaStreamSynchronize(stream);
+    if (live) { std::lock_guard<std::mutex> lock(live->mu); live->n--; }
     og_query_free_merge_state(merge_state);
     free_plan(plan);
     if (ev0) cudaEventDestroy(ev0);
@@ -359,7 +360,12 @@ OG_API int og_query_create(og_shard *s, const og_query_desc *d_in, og_query **ou
     if (d->n_filter > OG_MAX_FILTER) { set_error("filter too long (max %d items)", OG_MAX_FILTER); return OG_E_INVAL; }
     if (d->interval < 0 || d->tmin > d->tmax) { set_error("bad interval or time range"); return OG_E_INVAL; }
     std::unique_ptr<og_query> q(new og_query);
-    q->sh = s; q->desc = *d;
+    { /* waits while og_shard_append_files runs on the shard */
+        std::lock_guard<std::mutex> lock(s->live->mu);
+        s->live->n++;
+        q->sh = s; q->live = s->live;
+    }
+    q->desc = *d;
     q->calls.assign(d->calls, d->calls + d->n_calls);
     if (d->n_filter) q->filter.assign(d->filter, d->filter + d->n_filter);
     q->desc.calls = q->calls.data(); q->desc.filter = q->filter.data();

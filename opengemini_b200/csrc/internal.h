@@ -60,9 +60,12 @@ struct Scratch {
     template <class T> int get(T **p, size_t n) { int rc = dalloc(p, n); if (rc == OG_OK) bufs.push_back(*p); return rc; }
 };
 
-} // namespace ogpu
+/* the live queries of a shard: og_query_create counts up, ~og_query down, og_shard_append_files holds `mu` throughout.  Shared by
+ * the shard and its queries, so a query destroyed after its shard was closed still finds it. */
+struct LiveQueries { std::mutex mu; uint32_t n = 0; };
 
-struct og_shard {
+/* everything that describes a shard's rows and where they live: og_shard_append_files builds a new one and swaps it in whole */
+struct ShardState {
     int device = 0;
     uint8_t *d_data = nullptr; uint64_t data_len = 0; bool owns_data = true;
     uint32_t n_series = 0, n_segments = 0, n_columns = 0;
@@ -71,6 +74,7 @@ struct og_shard {
     uint64_t n_rows = 0, page_bytes = 0;
     uint64_t snappy_pages = 0, snappy_bytes_in = 0, snappy_bytes_out = 0; /* Snappy pages transcoded to raw at open */
     og_merge_info merge{1, 0, 0, 0, 0, 0, 0, 0, 0, 0}; /* og_shard_open_files (merge.cu); one file and zeros otherwise */
+    bool rows_merged = false; /* some open or append re-encoded a span: the Snappy counters were dropped with the file set's region */
     int64_t tmin = 0, tmax = 0;
     std::vector<uint64_t> sids;
     std::vector<int32_t> col_types;
@@ -84,6 +88,11 @@ struct og_shard {
     uint64_t *d_page_off = nullptr;         /* [(n_columns+1) * n_segments], time column last */
     uint32_t *d_page_len = nullptr;
     uint64_t *d_sids = nullptr;
+};
+
+} // namespace ogpu
+
+struct og_shard : ogpu::ShardState {
     /* materialise scratch for og_decode_segment (host pinned + device) */
     void *h_seg_buf = nullptr; size_t h_seg_buf_bytes = 0;
     void *d_seg_buf = nullptr; size_t d_seg_buf_bytes = 0;
@@ -99,6 +108,7 @@ struct og_shard {
                    uint64_t n_words = 0, n_packed = 0; /* words of the copy; segments stored as packed XOR deltas */ double build_ms = 0; };
     std::vector<IlCol> il; /* [n_columns] */
     std::mutex il_mu;      /* queries of one shard may be planned from different threads: the build is serialised */
+    std::shared_ptr<ogpu::LiveQueries> live = std::make_shared<ogpu::LiveQueries>();
     ~og_shard() {
         using ogpu::dev_free_all;
         if (owns_data) dev_free_all(d_data);
@@ -131,6 +141,7 @@ struct QueryP { /* passed by value to kernels */
 
 struct og_query {
     og_shard *sh = nullptr;
+    std::shared_ptr<ogpu::LiveQueries> live; /* the shard's live-query count, which this query is part of */
     og_query_desc desc{};
     std::vector<og_call> calls;
     std::vector<og_filter_item> filter;

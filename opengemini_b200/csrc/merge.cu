@@ -21,6 +21,13 @@
  *                           written into 1000-row segment slots (lib/util/util.go:72)
  *          encode_pages     the adaptive encoders of og_encode_pages (encode.cu), raw page for a float segment Gorilla refuses
  *   finish the new pages are appended behind the data, the directory is rebuilt, and shard_finalize validates the result.
+ *
+ * og_shard_append_files: files flushed into an open shard (DESIGN.md (d) "Appending flushed files").  The new files go through the
+ * same checks, directory build and upload; k_append_probe gives the shard's last time and span bounds per touched series; the
+ * spans' source pages are gathered and merged by merge_spans; k_append_splice builds the new directory from runs of the shard's,
+ * the files' and the merge's segments, and k_append_gather copies the live pages into a new data region.  Its copy loop is not
+ * shared with k_tssp_gather: the writer's CRC needs each lane to own one contiguous slice of a page, the gather deals 16-byte blocks
+ * out across the lanes so that a warp's loads and stores are consecutive.
  */
 #include <algorithm>
 #include <cstdio>
@@ -162,20 +169,24 @@ static SrcDir dir_of(const og_shard *s) {
 struct Span {
     uint32_t series;                 /* union series index */
     std::vector<uint32_t> src;       /* source segments, file-sequence order */
+    std::vector<uint32_t> src_file, src_rows; /* per source segment: its file (one file never repeats a time) and its rows */
     uint64_t rows = 0;
     uint32_t batch = 0, first_new = 0, n_new = 0; /* new segments [first_new, first_new + n_new) of batch `batch` */
 };
 struct NewSegs { /* what one batch produced, on the host */
     std::vector<uint64_t> off; std::vector<uint32_t> len; /* [(n_cols+1) * n] relative to the batch blob */
     std::vector<int64_t> tmin, tmax;
+    std::vector<uint32_t> rows;
     uint8_t *blob = nullptr; uint64_t bytes = 0; uint64_t base = 0; /* blob position in the final data */
     uint32_t n = 0;
 };
 
-/* Merge every span on the device, batch by batch.  Fills batches[] and each span's new-segment range. */
-static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const std::vector<uint32_t> &src_file, const std::vector<uint64_t> &sids, std::vector<NewSegs> &batches,
-                       Scratch &blobs, uint64_t *replaced_out) {
-    const uint32_t nc = src->n_columns, ncol1 = nc + 1;
+/* Merge every span on the device, batch by batch: the spans' source segments are read through `dir`, whose columns are `types` /
+ * `names`.  Fills batches[] and each span's new-segment range.  A repeated time names its file, or the shard's rows when the file
+ * is `shard_file`.  Every batch's blob is followed by 1024 readable bytes (k_append_gather reads past a page's end). */
+static int merge_spans(const SrcDir &dir, const std::vector<int32_t> &types, const std::vector<std::string> &names, const std::vector<Span *> &spans,
+                       const std::vector<uint64_t> &sids, uint32_t shard_file, std::vector<NewSegs> &batches, Scratch &blobs, uint64_t *replaced_out) {
+    const uint32_t nc = dir.n_columns, ncol1 = nc + 1;
     int rc;
     /* scratch per row: decode (8 t + 4 file + 4 span + 9 per column), sort (4 + 4 perm, 8 keys), heads + scan (8), output slots
        (8 + 9 per column), encoder staging and blob (2 x 8704 / 1000 per page) */
@@ -193,10 +204,7 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
     Scratch keep;
     if ((rc = keep.get(&d_rep, 1)) || (rc = keep.get(&d_err, 1)) || (rc = keep.get(&d_types, nc))) return rc;
     CU(cudaMemset(d_rep, 0, 8)); CU(cudaMemset(d_err, 0, sizeof(MergeErr)));
-    CU(cudaMemcpy(d_types, src->col_types.data(), nc * 4, cudaMemcpyHostToDevice));
-    std::vector<uint32_t> seg_rows(src->n_segments);
-    CU(cudaMemcpy(seg_rows.data(), src->d_seg_rows, (size_t)src->n_segments * 4, cudaMemcpyDeviceToHost));
-    const SrcDir dir = dir_of(src);
+    CU(cudaMemcpy(d_types, types.data(), nc * 4, cudaMemcpyHostToDevice));
     size_t sp0 = 0;
     while (sp0 < spans.size()) {
         size_t sp1 = sp0; uint64_t R64 = 0;
@@ -208,7 +216,8 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
         uint32_t row = 0;
         for (uint32_t k = 0; k < nsp; k++) {
             h_span_row0.push_back(row);
-            for (uint32_t g : spans[sp0 + k]->src) { h_seg.push_back(g); h_row0.push_back(row); h_file.push_back(src_file[g]); h_span.push_back(k); row += seg_rows[g]; }
+            const Span &sp = *spans[sp0 + k];
+            for (size_t j = 0; j < sp.src.size(); j++) { h_seg.push_back(sp.src[j]); h_row0.push_back(row); h_file.push_back(sp.src_file[j]); h_span.push_back(k); row += sp.src_rows[j]; }
         }
         h_span_row0.push_back(row);
         const uint32_t nsrc = (uint32_t)h_seg.size();
@@ -249,7 +258,8 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
         CU(cudaMemcpy(&he, d_err, sizeof he, cudaMemcpyDeviceToHost));
         if (he.code) {
             const unsigned long long sid = (unsigned long long)sids[spans[sp0 + he.span]->series];
-            if (he.code == M_STRING) { set_error("series sid %llu: string column \"%s\" has values in a span the merge re-encodes (there is no device string encoder)", sid, src->col_names[he.col].c_str()); return OG_E_UNSUPPORTED; }
+            if (he.code == M_STRING) { set_error("series sid %llu: string column \"%s\" has values in a span the merge re-encodes (there is no device string encoder)", sid, names[he.col].c_str()); return OG_E_UNSUPPORTED; }
+            if (he.code == M_REPEAT && (uint32_t)he.file == shard_file) { set_error("series sid %llu: time %lld appears twice in the shard's rows inside a merged span", sid, he.time); return OG_E_CORRUPT; }
             if (he.code == M_REPEAT) { set_error("series sid %llu: time %lld appears twice in file %d inside a merged span", sid, he.time, he.file); return OG_E_CORRUPT; }
             set_error("segment %d of the file set failed to decode (device code %d)", he.seg, he.code);
             return he.code == D_UNSUPPORTED ? OG_E_UNSUPPORTED : OG_E_CORRUPT;
@@ -274,7 +284,7 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
             (rc = b.get(&d_tmax, NS)) || (rc = b.get(&d_rows, NS)) || (rc = b.get(&d_cols, nc)))
             return rc;
         for (uint32_t c = 0; c < nc; c++)
-            if ((rc = b.get(&h_cols[c], out_rows * (src->col_types[c] == OG_TYPE_BOOL ? 1 : 8)))) return rc;
+            if ((rc = b.get(&h_cols[c], out_rows * (types[c] == OG_TYPE_BOOL ? 1 : 8)))) return rc;
         CU(cudaMemcpy(d_cols, h_cols.data(), nc * sizeof(uint8_t *), cudaMemcpyHostToDevice));
         CU(cudaMemcpy(seg_base, h_base.data(), nsp * 4ull, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(d_rows, h_rows.data(), NS * 4ull, cudaMemcpyHostToDevice));
@@ -290,9 +300,9 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
         ns.off.assign((size_t)ncol1 * NS, 0); ns.len.assign((size_t)ncol1 * NS, 0);
         for (uint32_t c = 0; c <= nc; c++) {
             const bool is_time = c == nc;
-            if (!is_time && src->col_types[c] == OG_TYPE_STRING) continue;
+            if (!is_time && types[c] == OG_TYPE_STRING) continue;
             uint64_t tot = 0;
-            rc = encode_pages(is_time ? OG_TYPE_INT : src->col_types[c], is_time ? 1 : 0, is_time ? (const void *)out_t : (const void *)h_cols[c],
+            rc = encode_pages(is_time ? OG_TYPE_INT : types[c], is_time ? 1 : 0, is_time ? (const void *)out_t : (const void *)h_cols[c],
                               is_time ? nullptr : out_ok + (size_t)c * out_rows, d_rows, NS, MERGE_RPS, blob + used, cap - used,
                               d_off + (size_t)c * NS, d_len + (size_t)c * NS, &tot, true);
             if (rc) return rc;
@@ -301,12 +311,13 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
             for (uint32_t g = 0; g < NS; g++) ns.off[(size_t)c * NS + g] += used;
             used += tot;
         }
-        ns.tmin.resize(NS); ns.tmax.resize(NS);
+        ns.tmin.resize(NS); ns.tmax.resize(NS); ns.rows = h_rows;
         CU(cudaMemcpy(ns.tmin.data(), d_tmin, NS * 8ull, cudaMemcpyDeviceToHost));
         CU(cudaMemcpy(ns.tmax.data(), d_tmax, NS * 8ull, cudaMemcpyDeviceToHost));
         /* keep only the bytes written: the batch's scratch goes back to the pool before the next batch */
-        if ((rc = blobs.get(&ns.blob, used))) return rc;
+        if ((rc = blobs.get(&ns.blob, used + 1024))) return rc;
         CU(cudaMemcpy(ns.blob, blob, used, cudaMemcpyDeviceToDevice));
+        CU(cudaMemset(ns.blob + used, 0, 1024));
         ns.bytes = used;
         batches.push_back(std::move(ns));
         sp0 = sp1;
@@ -317,24 +328,14 @@ static int merge_spans(og_shard *src, const std::vector<Span *> &spans, const st
     return OG_OK;
 }
 
-} // namespace ogpu
-
-using namespace ogpu;
-
-extern "C" {
-
-OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, og_shard **out) {
-    if (!files || !out || n_files == 0) { set_error("null argument or no files"); return OG_E_INVAL; }
-    *out = nullptr;
-    int rc = ensure_device(); if (rc) return rc;
-    int dev = 0; CU(cudaGetDevice(&dev));
-    auto is_ooo = [&](uint32_t f) { return file_flags && (file_flags[f] & OG_FILE_OUT_OF_ORDER); };
-    /* ---- checks, schema union by name (sorted), series union by sid (ascending) ---- */
-    std::map<std::string, int32_t> schema;
-    std::map<uint64_t, uint32_t> series_of_sid;
+/* The checks of every file description and the unions of a file set: columns by name (a column with two types is OG_E_TYPE) and
+ * series by sid.  `schema` may hold the columns of a shard the files join. */
+static int scan_files(const og_shard_desc *files, uint32_t n_files, const char *who, std::map<std::string, int32_t> &schema,
+                      std::map<uint64_t, uint32_t> &series_of_sid) {
+    int rc;
     for (uint32_t f = 0; f < n_files; f++) {
         const og_shard_desc *d = &files[f];
-        if (d->flags & OG_SHARD_DEVICE_DATA) { set_error("file %u: OG_SHARD_DEVICE_DATA is not accepted by og_shard_open_files (the files are copied into one buffer)", f); return OG_E_INVAL; }
+        if (d->flags & OG_SHARD_DEVICE_DATA) { set_error("file %u: OG_SHARD_DEVICE_DATA is not accepted by %s (the files are copied into one buffer)", f, who); return OG_E_INVAL; }
         if (d->data_len && !d->data) { set_error("file %u: null data", f); return OG_E_INVAL; }
         if ((rc = check_desc(d))) { char m[512]; snprintf(m, sizeof m, "%s", og_last_error()); set_error("file %u: %s", f, m); return rc; }
         std::map<std::string, int> seen;
@@ -354,58 +355,314 @@ OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_
         }
     }
     if (schema.size() > 64) { set_error("the files hold %zu distinct columns (limit 64)", schema.size()); return OG_E_INVAL; }
-    std::vector<std::string> names; std::vector<int32_t> types;
-    for (auto &kv : schema) { names.push_back(kv.first); types.push_back(kv.second); }
-    std::vector<uint64_t> sids;
-    for (auto &kv : series_of_sid) { kv.second = (uint32_t)sids.size(); sids.push_back(kv.first); }
-    const uint32_t nc = (uint32_t)names.size(), ncol1 = nc + 1, NSER = (uint32_t)sids.size();
-    /* ---- the source directory: every segment of every file, file by file, page offsets rebased into one buffer ---- */
-    std::vector<uint64_t> base(n_files), seg0(n_files + 1, 0), ser0(n_files + 1, 0);
+    return OG_OK;
+}
+
+/* every segment of every file, file by file, as one source directory over the union columns `names`; page offsets rebased into
+ * one buffer (file f at base[f]) */
+struct FileDir {
+    std::vector<uint64_t> base, seg0, ser0;
+    uint64_t data_len = 0;
+    uint32_t n = 0; /* segments */
+    std::vector<uint64_t> off; std::vector<uint32_t> len; /* [(n_columns + 1) * n], time last */
+    std::vector<int64_t> tmin, tmax;
+    std::vector<uint32_t> src_file, ssb; /* per segment: its file; per file series: its first segment */
+};
+static int build_file_dir(const og_shard_desc *files, uint32_t n_files, const std::vector<std::string> &names, FileDir &fd) {
+    const uint32_t nc = (uint32_t)names.size(), ncol1 = nc + 1;
+    fd.base.assign(n_files, 0); fd.seg0.assign(n_files + 1, 0); fd.ser0.assign(n_files + 1, 0);
     uint64_t data_len = 0;
     for (uint32_t f = 0; f < n_files; f++) {
-        base[f] = (data_len + 15) & ~15ull; data_len = base[f] + files[f].data_len;
-        seg0[f + 1] = seg0[f] + files[f].n_segments; ser0[f + 1] = ser0[f] + files[f].n_series;
+        fd.base[f] = (data_len + 15) & ~15ull; data_len = fd.base[f] + files[f].data_len;
+        fd.seg0[f + 1] = fd.seg0[f] + files[f].n_segments; fd.ser0[f + 1] = fd.ser0[f] + files[f].n_series;
     }
-    if (seg0[n_files] > 0xfffffff0ull) { set_error("too many segments"); return OG_E_INVAL; }
-    const uint32_t NSRC = (uint32_t)seg0[n_files];
-    std::vector<uint64_t> off((size_t)ncol1 * NSRC, 0); std::vector<uint32_t> len((size_t)ncol1 * NSRC, 0);
-    std::vector<int64_t> tmin(NSRC), tmax(NSRC);
-    std::vector<uint32_t> src_file(NSRC), ssb; ssb.reserve(ser0[n_files] + 1);
+    if (fd.seg0[n_files] > 0xfffffff0ull) { set_error("too many segments"); return OG_E_INVAL; }
+    fd.data_len = data_len;
+    const uint32_t NSRC = fd.n = (uint32_t)fd.seg0[n_files];
+    fd.off.assign((size_t)ncol1 * NSRC, 0); fd.len.assign((size_t)ncol1 * NSRC, 0);
+    fd.tmin.resize(NSRC); fd.tmax.resize(NSRC);
+    fd.src_file.resize(NSRC); fd.ssb.clear(); fd.ssb.reserve(fd.ser0[n_files] + 1);
     for (uint32_t f = 0; f < n_files; f++) {
         const og_shard_desc *d = &files[f];
         std::vector<int> col_of(d->n_columns);
         for (uint32_t c = 0; c < d->n_columns; c++) col_of[c] = (int)(std::lower_bound(names.begin(), names.end(), std::string(d->columns[c].name ? d->columns[c].name : "")) - names.begin());
         for (uint32_t g = 0; g < d->n_segments; g++) {
-            const size_t gs = seg0[f] + g;
-            src_file[gs] = f; tmin[gs] = d->seg_tmin[g]; tmax[gs] = d->seg_tmax[g];
+            const size_t gs = fd.seg0[f] + g;
+            fd.src_file[gs] = f; fd.tmin[gs] = d->seg_tmin[g]; fd.tmax[gs] = d->seg_tmax[g];
             for (uint32_t c = 0; c < d->n_columns; c++)
-                if (d->columns[c].page_len[g]) { off[(size_t)col_of[c] * NSRC + gs] = base[f] + d->columns[c].page_off[g]; len[(size_t)col_of[c] * NSRC + gs] = d->columns[c].page_len[g]; }
-            off[(size_t)nc * NSRC + gs] = base[f] + d->time_page_off[g]; len[(size_t)nc * NSRC + gs] = d->time_page_len[g];
+                if (d->columns[c].page_len[g]) { fd.off[(size_t)col_of[c] * NSRC + gs] = fd.base[f] + d->columns[c].page_off[g]; fd.len[(size_t)col_of[c] * NSRC + gs] = d->columns[c].page_len[g]; }
+            fd.off[(size_t)nc * NSRC + gs] = fd.base[f] + d->time_page_off[g]; fd.len[(size_t)nc * NSRC + gs] = d->time_page_len[g];
         }
-        for (uint32_t s = 0; s < d->n_series; s++) ssb.push_back((uint32_t)(seg0[f] + d->series_seg_begin[s]));
+        for (uint32_t s = 0; s < d->n_series; s++) fd.ssb.push_back((uint32_t)(fd.seg0[f] + d->series_seg_begin[s]));
     }
-    ssb.push_back(NSRC);
-    /* ---- per series: ordered segments in file order (no overlap across files), out-of-order segments, the span ---- */
-    std::vector<std::vector<uint32_t>> ordered(NSER), ooo(NSER);
-    std::vector<std::vector<uint32_t>> ord_file(NSER);
-    og_merge_info info{}; info.n_files = n_files;
+    fd.ssb.push_back(NSRC);
+    return OG_OK;
+}
+
+/* the files' bytes in one device buffer (one H2D per file) under the directory of build_file_dir, validated and with their Snappy
+ * pages transcoded (shard_finalize); fd.off / fd.len are updated to the transcoded directory, rows[] gets every segment's rows */
+static int upload_files(const og_shard_desc *files, uint32_t n_files, const std::vector<std::string> &names, const std::vector<int32_t> &types,
+                        int dev, FileDir &fd, std::unique_ptr<og_shard> &out, std::vector<uint32_t> &rows) {
+    int rc;
+    std::unique_ptr<og_shard> src(new og_shard);
+    src->device = dev; src->n_series = (uint32_t)fd.ser0[n_files]; src->n_segments = fd.n; src->n_columns = (uint32_t)names.size();
+    src->col_types = types; src->col_names = names; src->data_len = fd.data_len;
+    src->h_series_seg_begin = fd.ssb;
+    for (uint32_t f = 0; f < n_files; f++) src->sids.insert(src->sids.end(), files[f].sids, files[f].sids + files[f].n_series);
+    if ((rc = dalloc(&src->d_data, fd.data_len + 1024))) return rc;
+    CU(cudaMemset(src->d_data, 0, fd.data_len + 1024));
+    for (uint32_t f = 0; f < n_files; f++)
+        if (files[f].data_len) CU(cudaMemcpy(src->d_data + fd.base[f], files[f].data, files[f].data_len, cudaMemcpyHostToDevice));
+    if ((rc = upload_dir(src.get(), fd.ssb.data(), fd.tmin.data(), fd.tmax.data(), fd.off.data(), fd.len.data(), src->sids.data()))) return rc;
+    if ((rc = shard_finalize(src.get(), true))) return rc;
+    CU(cudaMemcpy(fd.off.data(), src->d_page_off, fd.off.size() * 8, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(fd.len.data(), src->d_page_len, fd.len.size() * 4, cudaMemcpyDeviceToHost));
+    rows.resize(fd.n);
+    CU(cudaMemcpy(rows.data(), src->d_seg_rows, fd.n * 4ull, cudaMemcpyDeviceToHost));
+    out = std::move(src);
+    return OG_OK;
+}
+
+static bool file_is_ooo(const uint32_t *file_flags, uint32_t f) { return file_flags && (file_flags[f] & OG_FILE_OUT_OF_ORDER); }
+
+/* per union series u: the files' ordered segments in file order and their out-of-order segments; ordered files that overlap in
+ * time for one series are OG_E_UNSUPPORTED.  Counts the out-of-order files into `info`. */
+static int split_segments(const og_shard_desc *files, uint32_t n_files, const uint32_t *file_flags, const FileDir &fd,
+                          std::map<uint64_t, uint32_t> &series_of_sid, const std::vector<uint64_t> &sids,
+                          std::vector<std::vector<uint32_t>> &ordered, std::vector<std::vector<uint32_t>> &ooo, og_merge_info &info) {
     for (uint32_t f = 0; f < n_files; f++) {
         const og_shard_desc *d = &files[f];
-        if (is_ooo(f)) info.n_out_of_order_files++;
+        const bool late = file_is_ooo(file_flags, f);
+        if (late) info.n_out_of_order_files++;
         for (uint32_t s = 0; s < d->n_series; s++) {
             const uint32_t u = series_of_sid[d->sids[s]];
             for (uint32_t g = d->series_seg_begin[s]; g < d->series_seg_begin[s + 1]; g++) {
-                const uint32_t gs = (uint32_t)(seg0[f] + g);
-                if (is_ooo(f)) { ooo[u].push_back(gs); continue; }
-                if (!ordered[u].empty() && tmin[gs] <= tmax[ordered[u].back()]) {
+                const uint32_t gs = (uint32_t)(fd.seg0[f] + g);
+                if (late) { ooo[u].push_back(gs); continue; }
+                if (!ordered[u].empty() && fd.tmin[gs] <= fd.tmax[ordered[u].back()]) {
                     set_error("series sid %llu: ordered files %u and %u overlap in time (%lld <= %lld); only out-of-order files may overlap",
-                              (unsigned long long)sids[u], src_file[ordered[u].back()], f, (long long)tmin[gs], (long long)tmax[ordered[u].back()]);
+                              (unsigned long long)sids[u], fd.src_file[ordered[u].back()], f, (long long)fd.tmin[gs], (long long)fd.tmax[ordered[u].back()]);
                     return OG_E_UNSUPPORTED;
                 }
                 ordered[u].push_back(gs);
             }
         }
     }
+    return OG_OK;
+}
+
+/* the hull [lo, hi] of a series' out-of-order segments */
+static void span_hull(const std::vector<uint32_t> &ooo, const FileDir &fd, int64_t *lo, int64_t *hi) {
+    *lo = INT64_MAX; *hi = INT64_MIN;
+    for (uint32_t g : ooo) { *lo = std::min(*lo, fd.tmin[g]); *hi = std::max(*hi, fd.tmax[g]); }
+}
+
+/* [a, b): the segments of a time-ordered list that [lo, hi] overlaps */
+static void span_bounds(const std::vector<uint32_t> &o, const FileDir &fd, int64_t lo, int64_t hi, uint32_t *a, uint32_t *b) {
+    uint32_t i = 0;
+    while (i < o.size() && fd.tmax[o[i]] < lo) i++;
+    *a = i;
+    while (i < o.size() && fd.tmin[o[i]] <= hi) i++;
+    *b = i;
+}
+
+/* oldest first: ordered files, then out-of-order files, each in file sequence (every out-of-order file is newer than every
+   ordered one, whatever their positions in files[]) */
+static void sort_oldest_first(std::vector<uint32_t> &segs, const FileDir &fd, const uint32_t *file_flags) {
+    auto rank = [&](uint32_t g) { return std::make_pair(file_is_ooo(file_flags, fd.src_file[g]) ? 1 : 0, fd.src_file[g]); };
+    std::stable_sort(segs.begin(), segs.end(), [&](uint32_t x, uint32_t y) { return rank(x) < rank(y); });
+}
+
+
+/* ---------------------------------------------------------------- og_shard_append_files */
+
+/* one source of spliced segments: a device directory whose column c is column col[c] of the source (-1: the source lacks it) */
+struct SegSrc {
+    const uint64_t *off; const uint32_t *len, *rows; const int64_t *tmin, *tmax;
+    const uint32_t *seg_region; uint32_t region; /* data region of segment i: seg_region[i], or `region` when seg_region is null */
+    const int32_t *col; uint32_t n_segments, n_columns;
+};
+enum { SRC_SHARD = 0, SRC_FILES = 1, SRC_MERGED = 2 };
+/* consecutive output segments [out0, next run's out0) of one series, from consecutive segments src0... of source `kind` */
+struct Run { uint32_t out0, src0, series, kind; };
+struct SpliceP {
+    SegSrc src[3];
+    const Run *runs; uint32_t n_runs, n_out, n_columns;
+    uint64_t *off; uint32_t *len, *rows, *series, *region; int64_t *tmin, *tmax; /* the output directory, [(n_columns + 1) * n_out] */
+};
+
+/* thread per output segment: its run, then its entries copied from the source, columns remapped (time column last) */
+__global__ void k_append_splice(SpliceP p) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= p.n_out) return;
+    uint32_t lo = 0, hi = p.n_runs;
+    while (hi - lo > 1) { const uint32_t m = (lo + hi) / 2; if (p.runs[m].out0 <= g) lo = m; else hi = m; }
+    const Run r = p.runs[lo];
+    const SegSrc &S = p.src[r.kind];
+    const uint32_t i = r.src0 + (g - r.out0);
+    p.tmin[g] = S.tmin[i]; p.tmax[g] = S.tmax[i]; p.rows[g] = S.rows[i]; p.series[g] = r.series;
+    p.region[g] = S.seg_region ? S.seg_region[i] : S.region;
+    for (uint32_t c = 0; c <= p.n_columns; c++) {
+        const int sc = c == p.n_columns ? (int)S.n_columns : S.col[c];
+        const size_t o = (size_t)c * p.n_out + g;
+        if (sc < 0) { p.off[o] = 0; p.len[o] = 0; continue; }
+        const size_t pi = (size_t)sc * S.n_segments + i;
+        p.off[o] = S.off[pi]; p.len[o] = S.len[pi];
+    }
+}
+
+/* sizes[n_pages] = 0, so the exclusive scan ends in the total */
+__global__ void k_append_sizes(const uint32_t *len, uint64_t n_pages, uint64_t *sizes) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i <= n_pages) sizes[i] = i < n_pages ? len[i] : 0;
+}
+
+constexpr int APPEND_GATHER_THREADS = 256;
+/* warp per page: the page from its region to its place in the new data region; dst_off becomes the page's offset there (0 for an
+ * absent page, as every directory has it).  The destination's 16-byte blocks are dealt out across the lanes (lane k writes blocks
+ * k, k + 32, ...), each fed by aligned 8-byte source loads shifted into place, so one step of the warp loads and stores 512
+ * consecutive bytes; the bytes before the first aligned block and after the last go one per lane.  Reads at most 7 bytes past a
+ * page: inside the 1024 bytes that follow every data region and blob. */
+__global__ void __launch_bounds__(APPEND_GATHER_THREADS) k_append_gather(const uint8_t *const *regions, const uint32_t *seg_region, const uint64_t *src_off,
+                                                                         const uint32_t *len, uint64_t *dst_off, uint32_t n_segments, uint64_t n_pages, uint8_t *out) {
+    const uint64_t page = ((uint64_t)blockIdx.x * APPEND_GATHER_THREADS + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    if (page >= n_pages) return;
+    const uint32_t l = len[page];
+    if (l == 0) { if (lane == 0) dst_off[page] = 0; return; }
+    const uint8_t *src = regions[seg_region[page % n_segments]] + src_off[page];
+    uint8_t *dst = out + dst_off[page];
+    const uint32_t head = min((uint32_t)((16 - ((uintptr_t)dst & 15)) & 15), l);
+    const uint32_t n_blocks = (l - head) / 16, tail = head + n_blocks * 16;
+    if (lane < head) dst[lane] = __ldg(src + lane);
+    for (uint32_t k = lane; k < n_blocks; k += 32) {
+        const uintptr_t sa = (uintptr_t)(src + head + 16 * k);
+        const uint64_t *q = (const uint64_t *)(sa & ~(uintptr_t)7);
+        const unsigned sh = (unsigned)(sa & 7) * 8;
+        uint64_t a = __ldg(q), b = __ldg(q + 1);
+        if (sh) { const uint64_t c = __ldg(q + 2); a = (a >> sh) | (b << (64 - sh)); b = (b >> sh) | (c << (64 - sh)); }
+        *(uint4 *)(dst + head + 16 * k) = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+    }
+    for (uint32_t i = tail + lane; i < l; i += 32) dst[i] = __ldg(src + i);
+}
+
+/* per probed series of the shard: its last time, and the range [a, b) of its segments that a span [lo, hi] overlaps */
+__global__ void k_append_probe(const uint32_t *series_seg_begin, const int64_t *seg_tmin, const int64_t *seg_tmax, const uint32_t *series,
+                               const int64_t *lo, const int64_t *hi, uint32_t n, int64_t *last, uint32_t *a_out, uint32_t *b_out) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const uint32_t g0 = series_seg_begin[series[k]], g1 = series_seg_begin[series[k] + 1];
+    last[k] = g1 > g0 ? seg_tmax[g1 - 1] : INT64_MIN;
+    uint32_t a = g0, e = g1; /* first segment with tmax >= lo (segments of a series are time-ordered) */
+    while (a < e) { const uint32_t m = (a + e) / 2; if (seg_tmax[m] < lo[k]) a = m + 1; else e = m; }
+    uint32_t b = a; e = g1;   /* first segment from a with tmin > hi */
+    while (b < e) { const uint32_t m = (b + e) / 2; if (seg_tmin[m] <= hi[k]) b = m + 1; else e = m; }
+    a_out[k] = a - g0; b_out[k] = b - g0;
+}
+
+/* the derived totals of a spliced directory: rows, page bytes, time pages that are neither const-delta nor one-row, the largest
+ * segment, the time range.  Reads only each time page's header. */
+__global__ void k_append_stats(const uint8_t *data, const uint64_t *off, const uint32_t *len, const uint32_t *rows, const int64_t *tmin,
+                               const int64_t *tmax, uint32_t n_segments, uint32_t n_columns, unsigned long long *tot, uint32_t *max_rows,
+                               long long *range, int *err) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= n_segments) return;
+    unsigned long long bytes = 0;
+    for (uint32_t c = 0; c <= n_columns; c++) bytes += len[(size_t)c * n_segments + g];
+    const size_t ti = (size_t)n_columns * n_segments + g;
+    TimeDesc t;
+    const int rc = parse_time_page(data + off[ti], len[ti], t);
+    if (rc != D_OK) { if (atomicCAS(err, 0, rc) == 0) err[1] = (int)g; return; }
+    atomicAdd(&tot[0], (unsigned long long)rows[g]);
+    atomicAdd(&tot[1], bytes);
+    if (t.kind != 0 && t.kind != 3) atomicAdd(&tot[2], 1ull);
+    atomicMax(max_rows, rows[g]);
+    atomicMin(&range[0], (long long)tmin[g]);
+    atomicMax(&range[1], (long long)tmax[g]);
+}
+
+/* a spliced directory and the data region its pages were gathered into */
+struct Spliced {
+    uint32_t n = 0, n_columns = 0;
+    uint64_t *off = nullptr; uint32_t *len = nullptr, *rows = nullptr, *series = nullptr; int64_t *tmin = nullptr, *tmax = nullptr;
+    uint8_t *data = nullptr; uint64_t data_len = 0;
+};
+/* k_append_splice over `runs`, then every referenced page copied from `regions` into one new buffer (+1024 zero bytes).  The
+ * directory arrays and the buffer are taken from `own`. */
+static int splice_and_gather(const SegSrc src[3], const std::vector<Run> &runs, uint32_t n_out, uint32_t n_columns,
+                             const std::vector<const uint8_t *> &regions, Scratch &own, Spliced &out) {
+    int rc;
+    const uint64_t n_pages = (uint64_t)(n_columns + 1) * n_out;
+    out.n = n_out; out.n_columns = n_columns;
+    Scratch tmp;
+    uint32_t *region; Run *d_runs; uint64_t *sizes; const uint8_t **d_regions;
+    if ((rc = own.get(&out.off, n_pages)) || (rc = own.get(&out.len, n_pages)) || (rc = own.get(&out.rows, n_out)) ||
+        (rc = own.get(&out.series, n_out)) || (rc = own.get(&out.tmin, n_out)) || (rc = own.get(&out.tmax, n_out)) ||
+        (rc = tmp.get(&region, n_out)) || (rc = tmp.get(&d_runs, runs.size())) || (rc = tmp.get(&sizes, n_pages + 1)) ||
+        (rc = tmp.get(&d_regions, regions.size())))
+        return rc;
+    CU(cudaMemcpy(d_regions, regions.data(), regions.size() * sizeof(void *), cudaMemcpyHostToDevice));
+    if (n_out) {
+        CU(cudaMemcpy(d_runs, runs.data(), runs.size() * sizeof(Run), cudaMemcpyHostToDevice));
+        SpliceP p;
+        for (int k = 0; k < 3; k++) p.src[k] = src[k];
+        p.runs = d_runs; p.n_runs = (uint32_t)runs.size(); p.n_out = n_out; p.n_columns = n_columns;
+        p.off = out.off; p.len = out.len; p.rows = out.rows; p.series = out.series; p.region = region; p.tmin = out.tmin; p.tmax = out.tmax;
+        k_append_splice<<<(n_out + 127) / 128, 128>>>(p);
+    }
+    k_append_sizes<<<(unsigned)((n_pages + 1 + 255) / 256), 256>>>(out.len, n_pages, sizes);
+    uint64_t *dst_off;
+    if ((rc = tmp.get(&dst_off, n_pages + 1))) return rc;
+    {
+        size_t tb = 0; void *t = nullptr;
+        CU(cub::DeviceScan::ExclusiveSum(nullptr, tb, sizes, dst_off, n_pages + 1));
+        if ((rc = tmp.get((uint8_t **)&t, tb))) return rc;
+        CU(cub::DeviceScan::ExclusiveSum(t, tb, sizes, dst_off, n_pages + 1));
+    }
+    CU(cudaGetLastError());
+    CU(cudaMemcpy(&out.data_len, dst_off + n_pages, 8, cudaMemcpyDeviceToHost));
+    if ((rc = own.get(&out.data, out.data_len + 1024))) return rc;
+    CU(cudaMemset(out.data + out.data_len, 0, 1024));
+    if (n_pages)
+        k_append_gather<<<(unsigned)((n_pages * 32 + APPEND_GATHER_THREADS - 1) / APPEND_GATHER_THREADS), APPEND_GATHER_THREADS>>>(
+            d_regions, region, out.off, out.len, dst_off, n_out, n_pages, out.data);
+    CU(cudaGetLastError());
+    CU(cudaMemcpy(out.off, dst_off, n_pages * 8, cudaMemcpyDeviceToDevice));
+    CU(cudaDeviceSynchronize()); /* tmp goes back to the pool */
+    return OG_OK;
+}
+
+} // namespace ogpu
+
+using namespace ogpu;
+
+extern "C" {
+
+OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, og_shard **out) {
+    if (!files || !out || n_files == 0) { set_error("null argument or no files"); return OG_E_INVAL; }
+    *out = nullptr;
+    int rc = ensure_device(); if (rc) return rc;
+    int dev = 0; CU(cudaGetDevice(&dev));
+    /* ---- checks, schema union by name (sorted), series union by sid (ascending) ---- */
+    std::map<std::string, int32_t> schema;
+    std::map<uint64_t, uint32_t> series_of_sid;
+    if ((rc = scan_files(files, n_files, "og_shard_open_files", schema, series_of_sid))) return rc;
+    std::vector<std::string> names; std::vector<int32_t> types;
+    for (auto &kv : schema) { names.push_back(kv.first); types.push_back(kv.second); }
+    std::vector<uint64_t> sids;
+    for (auto &kv : series_of_sid) { kv.second = (uint32_t)sids.size(); sids.push_back(kv.first); }
+    const uint32_t nc = (uint32_t)names.size(), ncol1 = nc + 1, NSER = (uint32_t)sids.size();
+    /* ---- the source directory: every segment of every file, file by file, page offsets rebased into one buffer ---- */
+    FileDir fd;
+    if ((rc = build_file_dir(files, n_files, names, fd))) return rc;
+    const uint32_t NSRC = fd.n;
+    std::vector<uint64_t> &off = fd.off; std::vector<uint32_t> &len = fd.len;
+    const std::vector<int64_t> &tmin = fd.tmin, &tmax = fd.tmax;
+    const std::vector<uint32_t> &src_file = fd.src_file;
+    /* ---- per series: ordered segments in file order (no overlap across files), out-of-order segments, the span ---- */
+    std::vector<std::vector<uint32_t>> ordered(NSER), ooo(NSER);
+    og_merge_info info{}; info.n_files = n_files;
+    if ((rc = split_segments(files, n_files, file_flags, fd, series_of_sid, sids, ordered, ooo, info))) return rc;
     /* layout of the output series: kept ordered segments before the span, the span, kept ones after it */
     std::vector<Span> span_store; span_store.reserve(NSER);
     std::vector<uint32_t> before(NSER), after_begin(NSER);
@@ -413,43 +670,26 @@ OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_
     for (uint32_t u = 0; u < NSER; u++) {
         const auto &o = ordered[u];
         if (ooo[u].empty()) { before[u] = after_begin[u] = (uint32_t)o.size(); continue; }
-        int64_t lo = INT64_MAX, hi = INT64_MIN;
-        for (uint32_t g : ooo[u]) { lo = std::min(lo, tmin[g]); hi = std::max(hi, tmax[g]); }
-        uint32_t a = 0, b;
-        while (a < o.size() && tmax[o[a]] < lo) a++;
-        b = a;
-        while (b < o.size() && tmin[o[b]] <= hi) b++;
+        int64_t lo, hi;
+        span_hull(ooo[u], fd, &lo, &hi);
+        uint32_t a, b;
+        span_bounds(o, fd, lo, hi, &a, &b);
         before[u] = a; after_begin[u] = b;
         Span sp; sp.series = u;
         sp.src.assign(o.begin() + a, o.begin() + b);
         sp.src.insert(sp.src.end(), ooo[u].begin(), ooo[u].end());
-        /* oldest first: ordered files, then out-of-order files, each in file sequence (every out-of-order file is newer than
-           every ordered one, whatever their positions in files[]) */
-        auto rank = [&](uint32_t g) { return std::make_pair(is_ooo(src_file[g]) ? 1 : 0, src_file[g]); };
-        std::stable_sort(sp.src.begin(), sp.src.end(), [&](uint32_t x, uint32_t y) { return rank(x) < rank(y); });
+        sort_oldest_first(sp.src, fd, file_flags);
         span_of[u] = (int)span_store.size();
         span_store.push_back(std::move(sp));
     }
-    /* ---- upload (one H2D per file), validate + transcode Snappy over the whole file set ---- */
-    std::unique_ptr<og_shard> src(new og_shard);
-    src->device = dev; src->n_series = (uint32_t)ser0[n_files]; src->n_segments = NSRC; src->n_columns = nc;
-    src->col_types = types; src->col_names = names; src->data_len = data_len;
-    src->h_series_seg_begin = ssb;
-    for (uint32_t f = 0; f < n_files; f++) src->sids.insert(src->sids.end(), files[f].sids, files[f].sids + files[f].n_series);
-    if ((rc = dalloc(&src->d_data, data_len + 1024))) return rc;
-    CU(cudaMemset(src->d_data, 0, data_len + 1024));
-    for (uint32_t f = 0; f < n_files; f++)
-        if (files[f].data_len) CU(cudaMemcpy(src->d_data + base[f], files[f].data, files[f].data_len, cudaMemcpyHostToDevice));
-    if ((rc = upload_dir(src.get(), ssb.data(), tmin.data(), tmax.data(), off.data(), len.data(), src->sids.data()))) return rc;
-    if ((rc = shard_finalize(src.get(), true))) return rc;
-    /* the transcoded directory and the row counts */
-    CU(cudaMemcpy(off.data(), src->d_page_off, off.size() * 8, cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(len.data(), src->d_page_len, len.size() * 4, cudaMemcpyDeviceToHost));
+    /* ---- upload (one H2D per file), validate + transcode Snappy over the whole file set; the transcoded directory and the row
+       counts come back ---- */
+    std::unique_ptr<og_shard> src;
     {
-        std::vector<uint32_t> rows(NSRC);
-        CU(cudaMemcpy(rows.data(), src->d_seg_rows, NSRC * 4ull, cudaMemcpyDeviceToHost));
+        std::vector<uint32_t> rows;
+        if ((rc = upload_files(files, n_files, names, types, dev, fd, src, rows))) return rc;
         for (auto &sp : span_store) {
-            for (uint32_t g : sp.src) sp.rows += rows[g];
+            for (uint32_t g : sp.src) { sp.rows += rows[g]; sp.src_file.push_back(src_file[g]); sp.src_rows.push_back(rows[g]); }
             info.series_merged++;
             info.segments_rewritten_in += sp.src.size();
         }
@@ -466,7 +706,7 @@ OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_
         std::vector<Span *> sp;
         for (auto &x : span_store) sp.push_back(&x);
         uint64_t replaced = 0;
-        if ((rc = merge_spans(src.get(), sp, src_file, sids, batches, blobs, &replaced))) return rc;
+        if ((rc = merge_spans(dir_of(src.get()), types, names, sp, sids, UINT32_MAX, batches, blobs, &replaced))) return rc;
         info.rows_replaced = replaced;
     }
     /* ---- final data: the file set's bytes, then the new pages of every batch ---- */
@@ -484,6 +724,7 @@ OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_
     }
     CU(cudaEventRecord(ev1, 0));
     if (batches.empty()) { s->snappy_pages = src->snappy_pages; s->snappy_bytes_in = src->snappy_bytes_in; s->snappy_bytes_out = src->snappy_bytes_out; }
+    s->rows_merged = !batches.empty();
     src.reset();
     /* ---- the output directory ---- */
     std::vector<uint32_t> o_ssb(NSER + 1, 0);
@@ -526,6 +767,275 @@ OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_
     info.rows_after_merge = s->n_rows;
     s->merge = info;
     *out = s.release();
+    return OG_OK;
+}
+
+OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files) {
+    if (!s || !files || n_files == 0) { set_error("null argument or no files"); return OG_E_INVAL; }
+    std::lock_guard<std::mutex> lock(s->live->mu); /* og_query_create waits until the append is done */
+    if (s->live->n) { set_error("%u queries on this shard are still open: destroy them before appending files", s->live->n); return OG_E_STATE; }
+    CU(cudaSetDevice(s->device));
+    int rc;
+    /* ---- checks; schema union with the shard's columns (sorted by name), series union with its sids (ascending) ---- */
+    const uint32_t onc = s->n_columns, ONSER = s->n_series, ONSEG = s->n_segments;
+    std::map<std::string, int32_t> schema;
+    for (uint32_t c = 0; c < onc; c++) schema[s->col_names[c]] = s->col_types[c];
+    if (schema.size() != onc) { set_error("the shard holds two columns of one name"); return OG_E_UNSUPPORTED; }
+    std::map<uint64_t, uint32_t> series_of_sid;
+    if ((rc = scan_files(files, n_files, "og_shard_append_files", schema, series_of_sid))) return rc;
+    std::map<uint64_t, uint32_t> old_of_sid;
+    for (uint32_t i = 0; i < ONSER; i++) {
+        if (!old_of_sid.emplace(s->sids[i], i).second) { set_error("the shard holds sid %llu twice", (unsigned long long)s->sids[i]); return OG_E_UNSUPPORTED; }
+        series_of_sid[s->sids[i]] = 0;
+    }
+    std::vector<std::string> names; std::vector<int32_t> types;
+    for (auto &kv : schema) { names.push_back(kv.first); types.push_back(kv.second); }
+    std::vector<uint64_t> sids;
+    for (auto &kv : series_of_sid) { kv.second = (uint32_t)sids.size(); sids.push_back(kv.first); }
+    const uint32_t nc = (uint32_t)names.size(), NSER = (uint32_t)sids.size();
+    std::vector<int32_t> col_of_old(nc, -1), identity(nc);
+    for (uint32_t c = 0; c < onc; c++) col_of_old[std::lower_bound(names.begin(), names.end(), s->col_names[c]) - names.begin()] = (int32_t)c;
+    for (uint32_t c = 0; c < nc; c++) identity[c] = (int32_t)c;
+    std::vector<int64_t> old_of(NSER, -1);
+    for (auto &kv : old_of_sid) old_of[series_of_sid[kv.first]] = kv.second;
+    /* ---- the new files' directory; per series their ordered segments (file order) and out-of-order segments ---- */
+    FileDir fd;
+    if ((rc = build_file_dir(files, n_files, names, fd))) return rc;
+    const uint32_t NN = fd.n;
+    std::vector<std::vector<uint32_t>> ordered(NSER), ooo(NSER);
+    og_merge_info info{}; info.n_files = n_files;
+    if ((rc = split_segments(files, n_files, file_flags, fd, series_of_sid, sids, ordered, ooo, info))) return rc;
+    /* ---- per series of the shard that takes new segments: its last time and the segments its span overlaps (device) ---- */
+    std::vector<uint32_t> probe_u, probe_old; std::vector<int64_t> probe_lo, probe_hi;
+    std::vector<int64_t> span_lo(NSER, INT64_MAX), span_hi(NSER, INT64_MIN);
+    for (uint32_t u = 0; u < NSER; u++) {
+        span_hull(ooo[u], fd, &span_lo[u], &span_hi[u]);
+        if (old_of[u] >= 0 && (!ordered[u].empty() || !ooo[u].empty())) {
+            probe_u.push_back(u); probe_old.push_back((uint32_t)old_of[u]); probe_lo.push_back(span_lo[u]); probe_hi.push_back(span_hi[u]);
+        }
+    }
+    const uint32_t NP = (uint32_t)probe_u.size();
+    std::vector<uint32_t> old_a(NSER, 0), old_b(NSER, 0);
+    {
+        Scratch t;
+        uint32_t *d_ser, *d_a, *d_b; int64_t *d_lo, *d_hi, *d_last;
+        if ((rc = t.get(&d_ser, NP)) || (rc = t.get(&d_lo, NP)) || (rc = t.get(&d_hi, NP)) || (rc = t.get(&d_last, NP)) || (rc = t.get(&d_a, NP)) || (rc = t.get(&d_b, NP))) return rc;
+        if (NP) {
+            CU(cudaMemcpy(d_ser, probe_old.data(), NP * 4ull, cudaMemcpyHostToDevice));
+            CU(cudaMemcpy(d_lo, probe_lo.data(), NP * 8ull, cudaMemcpyHostToDevice));
+            CU(cudaMemcpy(d_hi, probe_hi.data(), NP * 8ull, cudaMemcpyHostToDevice));
+            k_append_probe<<<(NP + 127) / 128, 128>>>(s->d_series_seg_begin, s->d_tmin, s->d_tmax, d_ser, d_lo, d_hi, NP, d_last, d_a, d_b);
+            CU(cudaGetLastError());
+            std::vector<int64_t> last(NP); std::vector<uint32_t> a(NP), b(NP);
+            CU(cudaMemcpy(last.data(), d_last, NP * 8ull, cudaMemcpyDeviceToHost));
+            CU(cudaMemcpy(a.data(), d_a, NP * 4ull, cudaMemcpyDeviceToHost));
+            CU(cudaMemcpy(b.data(), d_b, NP * 4ull, cudaMemcpyDeviceToHost));
+            for (uint32_t k = 0; k < NP; k++) {
+                const uint32_t u = probe_u[k];
+                /* the flush rule: a series' new ordered rows start after the last time the shard holds for it */
+                if (!ordered[u].empty() && fd.tmin[ordered[u][0]] <= last[k]) {
+                    set_error("series sid %llu: ordered file %u starts at %lld, not after the shard's last time %lld; only out-of-order files may overlap the shard",
+                              (unsigned long long)sids[u], fd.src_file[ordered[u][0]], (long long)fd.tmin[ordered[u][0]], (long long)last[k]);
+                    return OG_E_UNSUPPORTED;
+                }
+                old_a[u] = a[k]; old_b[u] = b[k];
+            }
+        }
+    }
+    /* ---- layout: per series the shard's segments then its new ordered ones (one time-ordered list of n_old + n_new); a span
+       rewrites the list's [before, after_begin) with the out-of-order segments ---- */
+    auto n_old = [&](uint32_t u) { return old_of[u] < 0 ? 0u : s->h_series_seg_begin[old_of[u] + 1] - s->h_series_seg_begin[old_of[u]]; };
+    auto g0_old = [&](uint32_t u) { return old_of[u] < 0 ? 0u : s->h_series_seg_begin[old_of[u]]; };
+    std::vector<uint32_t> before(NSER), after_begin(NSER);
+    std::vector<int> span_of(NSER, -1);
+    std::vector<Span> span_store;
+    for (uint32_t u = 0; u < NSER; u++) {
+        const uint32_t no = n_old(u);
+        const auto &o = ordered[u];
+        if (ooo[u].empty()) { before[u] = after_begin[u] = no + (uint32_t)o.size(); continue; }
+        uint32_t na, nb; /* the same bounds over the new ordered segments, which follow the shard's */
+        span_bounds(o, fd, span_lo[u], span_hi[u], &na, &nb);
+        before[u] = old_a[u] < no ? old_a[u] : no + na;
+        after_begin[u] = old_b[u] < no ? old_b[u] : no + nb;
+        Span sp; sp.series = u;
+        span_of[u] = (int)span_store.size();
+        span_store.push_back(std::move(sp));
+    }
+    /* ---- upload, validate and transcode the new files only ---- */
+    std::unique_ptr<og_shard> nw;
+    std::vector<uint32_t> new_rows;
+    if ((rc = upload_files(files, n_files, names, types, s->device, fd, nw, new_rows))) return rc;
+    /* the interleaved copies describe the old layout: dropped now, rebuilt by the first query that wants them */
+    {
+        std::lock_guard<std::mutex> il_lock(s->il_mu);
+        for (og_shard::IlCol &c : s->il)
+            dev_free_all(c.words, c.grp_off, c.grp_rows, c.grp_col, c.lane_seg, c.lane_rows, c.lane_series, c.lane_win, c.lane_t0, c.lane_dt, c.gen_list);
+        s->il.assign(s->n_columns, og_shard::IlCol{});
+    }
+    Scratch d_maps;
+    int32_t *d_col_old, *d_identity;
+    if ((rc = d_maps.get(&d_col_old, nc)) || (rc = d_maps.get(&d_identity, nc))) return rc;
+    CU(cudaMemcpy(d_col_old, col_of_old.data(), nc * 4ull, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_identity, identity.data(), nc * 4ull, cudaMemcpyHostToDevice));
+    SegSrc src[3] = {};
+    src[SRC_SHARD] = SegSrc{s->d_page_off, s->d_page_len, s->d_seg_rows, s->d_tmin, s->d_tmax, nullptr, 0, d_col_old, ONSEG, onc};
+    src[SRC_FILES] = SegSrc{nw->d_page_off, nw->d_page_len, nw->d_seg_rows, nw->d_tmin, nw->d_tmax, nullptr, 1, d_identity, NN, nc};
+    cudaEvent_t ev0, ev1;
+    CU(cudaEventCreate(&ev0)); CU(cudaEventCreate(&ev1));
+    struct FreeEv { cudaEvent_t a, b; ~FreeEv() { cudaEventDestroy(a); cudaEventDestroy(b); } } free_ev{ev0, ev1};
+    CU(cudaEventRecord(ev0, 0));
+    /* ---- merge: the spans' source pages gathered into one buffer (the shard's rows first, then the new files in sequence,
+       ordered before out-of-order), then merge_spans as at open ---- */
+    std::vector<NewSegs> batches;
+    Scratch blobs, msrc_own;
+    if (!span_store.empty()) {
+        std::vector<Run> runs;
+        uint32_t n_src = 0;
+        for (auto &sp : span_store) {
+            const uint32_t u = sp.series, no = n_old(u);
+            const auto &o = ordered[u];
+            const uint32_t ob = std::min(before[u], no), oe = std::min(after_begin[u], no);
+            if (oe > ob) { /* the shard's rows: one "file", older than every new one */
+                runs.push_back(Run{n_src, g0_old(u) + ob, 0, SRC_SHARD});
+                for (uint32_t k = 0; k < oe - ob; k++) { sp.src.push_back(n_src + k); sp.src_file.push_back(n_files); }
+                n_src += oe - ob;
+            }
+            std::vector<uint32_t> news;
+            for (uint32_t k = std::max(before[u], no); k < after_begin[u]; k++) news.push_back(o[k - no]);
+            news.insert(news.end(), ooo[u].begin(), ooo[u].end());
+            sort_oldest_first(news, fd, file_flags);
+            for (uint32_t g : news) {
+                runs.push_back(Run{n_src, g, 0, SRC_FILES});
+                sp.src.push_back(n_src++); sp.src_file.push_back(fd.src_file[g]);
+            }
+            info.series_merged++;
+            info.segments_rewritten_in += sp.src.size();
+        }
+        for (uint32_t u = 0; u < NSER; u++) for (uint32_t g : ooo[u]) info.out_of_order_rows += new_rows[g];
+        Spliced ms;
+        if ((rc = splice_and_gather(src, runs, n_src, nc, {s->d_data, nw->d_data}, msrc_own, ms))) return rc;
+        { /* the rows of every source segment, spliced with the rest of its directory: one copy */
+            std::vector<uint32_t> rows(n_src);
+            CU(cudaMemcpy(rows.data(), ms.rows, n_src * 4ull, cudaMemcpyDeviceToHost));
+            for (auto &sp : span_store)
+                for (uint32_t i : sp.src) { sp.src_rows.push_back(rows[i]); sp.rows += rows[i]; }
+        }
+        SrcDir dir;
+        dir.data = ms.data; dir.page_off = ms.off; dir.page_len = ms.len; dir.seg_rows = ms.rows; dir.n_segments = ms.n; dir.n_columns = nc;
+        std::vector<Span *> sp;
+        for (auto &x : span_store) sp.push_back(&x);
+        uint64_t replaced = 0;
+        if ((rc = merge_spans(dir, types, names, sp, sids, n_files, batches, blobs, &replaced))) return rc;
+        info.rows_replaced = replaced;
+    }
+    /* ---- the merged segments as one source directory, each batch's blob its own region ---- */
+    std::vector<uint32_t> m_first(batches.size() + 1, 0);
+    for (size_t b = 0; b < batches.size(); b++) m_first[b + 1] = m_first[b] + batches[b].n;
+    const uint32_t NM = m_first[batches.size()];
+    std::vector<const uint8_t *> regions = {s->d_data, nw->d_data};
+    Scratch m_own;
+    if (NM) {
+        std::vector<uint64_t> off((size_t)(nc + 1) * NM); std::vector<uint32_t> len((size_t)(nc + 1) * NM), rows(NM), reg(NM);
+        std::vector<int64_t> tmin(NM), tmax(NM);
+        for (size_t b = 0; b < batches.size(); b++) {
+            const NewSegs &B = batches[b];
+            regions.push_back(B.blob);
+            for (uint32_t g = 0; g < B.n; g++) {
+                const uint32_t m = m_first[b] + g;
+                for (uint32_t c = 0; c <= nc; c++) { off[(size_t)c * NM + m] = B.off[(size_t)c * B.n + g]; len[(size_t)c * NM + m] = B.len[(size_t)c * B.n + g]; }
+                rows[m] = B.rows[g]; reg[m] = 2 + (uint32_t)b; tmin[m] = B.tmin[g]; tmax[m] = B.tmax[g];
+            }
+        }
+        SegSrc &m = src[SRC_MERGED];
+        uint64_t *d_off; uint32_t *d_len, *d_rows, *d_reg; int64_t *d_tmin, *d_tmax;
+        if ((rc = m_own.get(&d_off, off.size())) || (rc = m_own.get(&d_len, len.size())) || (rc = m_own.get(&d_rows, NM)) || (rc = m_own.get(&d_reg, NM)) ||
+            (rc = m_own.get(&d_tmin, NM)) || (rc = m_own.get(&d_tmax, NM)))
+            return rc;
+        CU(cudaMemcpy(d_off, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(d_len, len.data(), len.size() * 4, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(d_rows, rows.data(), NM * 4ull, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(d_reg, reg.data(), NM * 4ull, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(d_tmin, tmin.data(), NM * 8ull, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(d_tmax, tmax.data(), NM * 8ull, cudaMemcpyHostToDevice));
+        m = SegSrc{d_off, d_len, d_rows, d_tmin, d_tmax, d_reg, 0, d_identity, NM, nc};
+    }
+    /* ---- the new directory as runs: per series the shard's segments before its span, new ordered ones before it, the span's
+       merged segments, then the rest of both ---- */
+    std::vector<Run> runs;
+    std::vector<uint32_t> o_ssb(NSER + 1, 0);
+    uint32_t NOUT = 0;
+    auto emit = [&](uint32_t u, uint32_t k0, uint32_t k1) { /* positions [k0, k1) of series u's time-ordered list */
+        const uint32_t no = n_old(u);
+        if (std::min(k1, no) > k0) { runs.push_back(Run{NOUT, g0_old(u) + k0, u, SRC_SHARD}); NOUT += std::min(k1, no) - k0; }
+        for (uint32_t k = std::max(k0, no); k < k1; k++) runs.push_back(Run{NOUT++, ordered[u][k - no], u, SRC_FILES});
+        info.segments_kept += k1 - k0;
+    };
+    for (uint32_t u = 0; u < NSER; u++) {
+        o_ssb[u] = NOUT;
+        const uint32_t total = n_old(u) + (uint32_t)ordered[u].size();
+        emit(u, 0, before[u]);
+        if (span_of[u] >= 0) {
+            const Span &sp = span_store[span_of[u]];
+            if (sp.n_new) { runs.push_back(Run{NOUT, m_first[sp.batch] + sp.first_new, u, SRC_MERGED}); NOUT += sp.n_new; }
+            info.segments_rewritten_out += sp.n_new;
+        }
+        emit(u, after_begin[u], total);
+    }
+    o_ssb[NSER] = NOUT;
+    /* ---- gather the live pages into the new data region ---- */
+    std::unique_ptr<og_shard> out(new og_shard);
+    Scratch out_own;
+    Spliced sd;
+    if ((rc = splice_and_gather(src, runs, NOUT, nc, regions, out_own, sd))) return rc;
+    CU(cudaEventRecord(ev1, 0));
+    /* ---- derived state ---- */
+    {
+        Scratch t;
+        unsigned long long *d_tot; uint32_t *d_max; long long *d_range; int *d_err;
+        if ((rc = t.get(&d_tot, 3)) || (rc = t.get(&d_max, 1)) || (rc = t.get(&d_range, 2)) || (rc = t.get(&d_err, 2))) return rc;
+        const long long r0[2] = {INT64_MAX, INT64_MIN};
+        CU(cudaMemset(d_tot, 0, 24)); CU(cudaMemset(d_max, 0, 4)); CU(cudaMemset(d_err, 0, 8));
+        CU(cudaMemcpy(d_range, r0, 16, cudaMemcpyHostToDevice));
+        if (NOUT) k_append_stats<<<(NOUT + 127) / 128, 128>>>(sd.data, sd.off, sd.len, sd.rows, sd.tmin, sd.tmax, NOUT, nc, d_tot, d_max, d_range, d_err);
+        CU(cudaGetLastError());
+        unsigned long long tot[3]; long long range[2]; int err[2];
+        CU(cudaMemcpy(tot, d_tot, 24, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(&out->max_seg_rows, d_max, 4, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(range, d_range, 16, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(err, d_err, 8, cudaMemcpyDeviceToHost));
+        if (err[0]) { set_error("segment %d: time page failed to parse after the append (device code %d)", err[1], err[0]); return OG_E_CORRUPT; }
+        out->n_rows = tot[0]; out->page_bytes = tot[1]; out->irregular_time_pages = tot[2]; out->tmin = range[0]; out->tmax = range[1];
+    }
+    /* the Snappy counters follow og_shard_open_files over the whole set: a merge there drops them */
+    out->rows_merged = s->rows_merged || !batches.empty();
+    if (!out->rows_merged) {
+        out->snappy_pages = s->snappy_pages + nw->snappy_pages;
+        out->snappy_bytes_in = s->snappy_bytes_in + nw->snappy_bytes_in; out->snappy_bytes_out = s->snappy_bytes_out + nw->snappy_bytes_out;
+    }
+    out->page_bytes = out->page_bytes - out->snappy_bytes_out + out->snappy_bytes_in;
+    /* ---- the new state, complete and synchronised before it is swapped in: nothing fails after the swap ---- */
+    out->device = s->device; out->n_series = NSER; out->n_segments = NOUT; out->n_columns = nc;
+    out->sids = sids; out->col_types = types; out->col_names = names; out->h_series_seg_begin = o_ssb;
+    if ((rc = dalloc(&out->d_series_seg_begin, (size_t)NSER + 1)) || (rc = dalloc(&out->d_sids, (size_t)NSER))) return rc;
+    CU(cudaMemcpy(out->d_series_seg_begin, o_ssb.data(), ((size_t)NSER + 1) * 4, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(out->d_sids, sids.data(), (size_t)NSER * 8, cudaMemcpyHostToDevice));
+    float ms = 0;
+    CU(cudaEventElapsedTime(&ms, ev0, ev1));
+    info.merge_ms = ms;
+    info.rows_after_merge = out->n_rows;
+    auto take = [](Scratch &own, void *p) { own.bufs.erase(std::find(own.bufs.begin(), own.bufs.end(), p)); };
+    for (void *p : {(void *)sd.off, (void *)sd.len, (void *)sd.rows, (void *)sd.series, (void *)sd.tmin, (void *)sd.tmax, (void *)sd.data}) take(out_own, p);
+    out->d_page_off = sd.off; out->d_page_len = sd.len; out->d_seg_rows = sd.rows; out->d_seg_series = sd.series; out->d_tmin = sd.tmin; out->d_tmax = sd.tmax;
+    out->d_data = sd.data; out->data_len = sd.data_len; out->owns_data = true;
+    out->merge = info;
+    CU(cudaDeviceSynchronize());
+    /* swap the whole state: `out` takes the old one and frees it on return (the caller's buffer of a shard opened in place is not
+       freed) */
+    std::swap(static_cast<ShardState &>(*s), static_cast<ShardState &>(*out));
+    {
+        std::lock_guard<std::mutex> il_lock(s->il_mu);
+        s->il.assign(s->n_columns, og_shard::IlCol{});
+    }
     return OG_OK;
 }
 

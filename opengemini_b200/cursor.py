@@ -93,11 +93,9 @@ class Shard:
         L.check(L.lib().og_shard_open(C.byref(d), C.byref(h)), "og_shard_open")
         return cls(h.value)
 
-    @classmethod
-    def open_files(cls, files):
-        """One shard from its ordered and out-of-order files (og_shard_open_files): files = [(desc_or_tssp_bytes, out_of_order)]
-        in file-sequence order, oldest first.  A file is an L.ShardDesc (Shard.desc) or a TSSP file image, which goes through
-        og_tssp_parse / og_tssp_desc.  Overlapping rows are merged on the device as the shard opens; merge_info() reports it."""
+    @staticmethod
+    def _with_file_descs(files, call):
+        """files = [(desc_or_tssp_bytes, out_of_order)] -> call(descs, flags) with every TSSP image parsed for the call's length."""
         descs = (L.ShardDesc * len(files))()
         flags = np.array([L.FILE_OUT_OF_ORDER if ooo else 0 for _f, ooo in files], dtype=np.uint32)
         keep, parsed = [], []
@@ -112,12 +110,30 @@ class Shard:
                 L.check(L.lib().og_tssp_parse(buf.ctypes.data, buf.size, C.byref(t)), "og_tssp_parse")
                 parsed.append(t)
                 L.check(L.lib().og_tssp_desc(t, C.byref(descs[i])), "og_tssp_desc")
-            h = C.c_void_p()
-            L.check(L.lib().og_shard_open_files(descs, _ptr(flags, C.c_uint32), len(files), C.byref(h)), "og_shard_open_files")
+            return call(descs, flags)
         finally:
             for t in parsed:
                 L.lib().og_tssp_free(t)
+
+    @classmethod
+    def open_files(cls, files):
+        """One shard from its ordered and out-of-order files (og_shard_open_files): files = [(desc_or_tssp_bytes, out_of_order)]
+        in file-sequence order, oldest first.  A file is an L.ShardDesc (Shard.desc) or a TSSP file image, which goes through
+        og_tssp_parse / og_tssp_desc.  Overlapping rows are merged on the device as the shard opens; merge_info() reports it."""
+        h = C.c_void_p()
+
+        def call(descs, flags):
+            L.check(L.lib().og_shard_open_files(descs, _ptr(flags, C.c_uint32), len(files), C.byref(h)), "og_shard_open_files")
+        cls._with_file_descs(files, call)
         return cls(h.value)
+
+    def append_files(self, files):
+        """Files flushed after the shard was built (og_shard_append_files), in the form open_files takes, oldest first.  The shard
+        then answers as open_files over its files followed by these.  Series and column indices may move: rebuild group maps."""
+        def call(descs, flags):
+            L.check(L.lib().og_shard_append_files(self.h, descs, _ptr(flags, C.c_uint32), len(files)), "og_shard_append_files")
+        self._with_file_descs(files, call)
+        return self
 
     def merge_info(self):
         m = L.MergeInfo()
