@@ -277,7 +277,8 @@ OG_API int og_shard_info(const og_shard *s, uint64_t *n_series, uint64_t *n_segm
  * the older one's when that is null.  The schema is the union of the field columns by name, sorted by name (record.go:438-466); a
  * column a file lacks is null for its rows.  Series are the union by sid, ascending.
  * Only the rows of a series around its out-of-order rows are re-encoded (1000-row segments, the encoders of og_encode_pages; a
- * float segment the Gorilla encoder refuses gets a raw page): ordered segments outside that span keep their bytes.
+ * float segment the Gorilla encoder refuses gets a raw page): ordered segments outside that span keep their bytes.  The shard's
+ * data region holds the pages its directory references; without out-of-order rows it is the files' bytes as they were copied in.
  * Refused: a column with two types (OG_E_TYPE), ordered files that overlap in time for one series, a string column with values
  * inside a re-encoded span (OG_E_UNSUPPORTED), a time repeated within one file's series inside a span (OG_E_CORRUPT).
  * WHERE applies to the merged row (the reference filters each file before the merge: DESIGN.md "Deviations"). ---- */
@@ -291,9 +292,9 @@ typedef struct og_merge_info {
     uint64_t rows_after_merge;
     uint64_t segments_kept;          /* ordered segments carried over byte for byte */
     uint64_t segments_rewritten_in, segments_rewritten_out;
-    double merge_ms;                 /* elapsed time of the merge phase, from the first batch to the assembled data region (CUDA events
-                                        on the legacy stream; includes the host work between batches and the device-to-device copy
-                                        of the file set's data region) */
+    double merge_ms;                 /* elapsed time of the merge phase, from the splice of the spans' source segments to the gather
+                                        of the live pages into the new data region (CUDA events on the legacy stream; includes the
+                                        host work between batches) */
 } og_merge_info;
 OG_API int og_shard_merge_info(const og_shard *s, og_merge_info *out); /* og_shard_open / og_shard_synth shards: n_files = 1, zeros;
                                                                          after og_shard_append_files: that call's files and counters */

@@ -1,18 +1,24 @@
 /*
- * merge.cu — og_shard_open_files: the ordered and out-of-order files of one shard opened as ONE og_shard.
+ * merge.cu — TSSP files into a shard (DESIGN.md (d) "Bringing files into a shard").  og_shard_open_files opens the ordered and
+ * out-of-order files of one shard as ONE og_shard; og_shard_append_files adds files flushed into an open shard.  An open is an
+ * append to an empty shard: both run add_files.
  *
  * The reference merges a shard's files for every series of every query (include/ogpu.h lists the code).  Here the merge runs
- * once, when the shard is opened:
+ * once, when the files join the shard:
  *
- *   host   check every description (check_desc), union of columns by name and of series by sid, the ordered segments of a
- *          series in file order (overlapping ordered files are refused), one H2D per file into one data buffer with rebased
- *          page offsets; the whole file set is validated and its Snappy pages transcoded by shard_finalize, so the merge only
- *          sees codecs ColIter / TimeIter decode.
- *   order  the rows of one time are ranked oldest first: ordered files, then out-of-order files, each in file sequence.
- *   span   per series with out-of-order rows: the hull [min, max] of its out-of-order segments' time ranges, widened to the
- *          ordered segments it overlaps.  Those ordered segments and every out-of-order segment of the series are rewritten;
- *          every other segment keeps its bytes and its directory entry.
- *   device per batch of spans (scratch ~ rows in the batch, under a device-memory budget):
+ *   host   check every description (check_desc), union of columns by name and of series by sid with the shard's, the ordered
+ *          segments of a series in file order (overlapping ordered files are refused), one H2D per file into one data buffer with
+ *          rebased page offsets; the new files are validated and their Snappy pages transcoded by shard_finalize, so the merge only
+ *          sees codecs ColIter / TimeIter decode.  The shard's own pages are not validated again.
+ *   probe  k_append_probe: per series of the shard that takes new segments, its last time (a new ordered segment must start after
+ *          it) and the range of its segments a span overlaps.
+ *   order  the rows of one time are ranked oldest first: the shard's rows, then ordered files, then out-of-order files, each in
+ *          file sequence.
+ *   span   per series with out-of-order rows: the hull [min, max] of its out-of-order segments' time ranges, widened to the shard's
+ *          and the new ordered segments it overlaps.  Those segments and every out-of-order segment of the series are rewritten;
+ *          every other segment keeps its bytes.
+ *   device the spans' source segments spliced into one directory (k_append_splice, k_append_gather), then per batch of spans
+ *          (scratch ~ rows in the batch, under a device-memory budget):
  *          k_merge_decode   one thread per source segment: rows of every union column, laid out span by span, sources of a span
  *                           in file-sequence order
  *          StableSortPairs  by time inside each span (cub segmented sort): rows of equal time stay in file order, oldest first
@@ -20,14 +26,13 @@
  *          k_merge_combine  one thread per run: each column takes its newest non-null value (mergeRecRow, record.go:468-505),
  *                           written into 1000-row segment slots (lib/util/util.go:72)
  *          encode_pages     the adaptive encoders of og_encode_pages (encode.cu), raw page for a float segment Gorilla refuses
- *   finish the new pages are appended behind the data, the directory is rebuilt, and shard_finalize validates the result.
+ *   finish k_append_splice builds the new directory from runs of the shard's, the files' and the merge's segments; k_append_gather
+ *          copies the live pages into a new data region, unless the files' region already holds every one of them (nothing merged
+ *          and no older segments), which is then kept as it is; k_append_stats derives the shard's totals from the time pages'
+ *          headers, and the new state is swapped in whole.
  *
- * og_shard_append_files: files flushed into an open shard (DESIGN.md (d) "Appending flushed files").  The new files go through the
- * same checks, directory build and upload; k_append_probe gives the shard's last time and span bounds per touched series; the
- * spans' source pages are gathered and merged by merge_spans; k_append_splice builds the new directory from runs of the shard's,
- * the files' and the merge's segments, and k_append_gather copies the live pages into a new data region.  Its copy loop is not
- * shared with k_tssp_gather: the writer's CRC needs each lane to own one contiguous slice of a page, the gather deals 16-byte blocks
- * out across the lanes so that a warp's loads and stores are consecutive.
+ * The gather's copy loop is not shared with k_tssp_gather: the writer's CRC needs each lane to own one contiguous slice of a page,
+ * the gather deals 16-byte blocks out across the lanes so that a warp's loads and stores are consecutive.
  */
 #include <algorithm>
 #include <cstdio>
@@ -158,12 +163,9 @@ __global__ void k_merge_combine(const int64_t *t, const uint32_t *perm, const ui
     if (slot == MERGE_RPS - 1 || local == cnt - 1) seg_tmax[g] = tt;
 }
 
-static SrcDir dir_of(const og_shard *s) {
-    SrcDir d;
-    d.data = s->d_data; d.page_off = s->d_page_off; d.page_len = s->d_page_len; d.seg_rows = s->d_seg_rows;
-    d.n_segments = s->n_segments; d.n_columns = s->n_columns;
-    return d;
-}
+enum { SRC_SHARD = 0, SRC_FILES = 1, SRC_MERGED = 2 };
+/* consecutive output segments [out0, next run's out0) of one series, from consecutive segments src0... of source `kind` */
+struct Run { uint32_t out0, src0, series, kind; };
 
 /* a rewritten span: source segments (file order) -> new segments */
 struct Span {
@@ -177,15 +179,17 @@ struct NewSegs { /* what one batch produced, on the host */
     std::vector<uint64_t> off; std::vector<uint32_t> len; /* [(n_cols+1) * n] relative to the batch blob */
     std::vector<int64_t> tmin, tmax;
     std::vector<uint32_t> rows;
-    uint8_t *blob = nullptr; uint64_t bytes = 0; uint64_t base = 0; /* blob position in the final data */
+    uint8_t *blob = nullptr; uint64_t bytes = 0;
     uint32_t n = 0;
 };
 
 /* Merge every span on the device, batch by batch: the spans' source segments are read through `dir`, whose columns are `types` /
- * `names`.  Fills batches[] and each span's new-segment range.  A repeated time names its file, or the shard's rows when the file
- * is `shard_file`.  Every batch's blob is followed by 1024 readable bytes (k_append_gather reads past a page's end). */
-static int merge_spans(const SrcDir &dir, const std::vector<int32_t> &types, const std::vector<std::string> &names, const std::vector<Span *> &spans,
-                       const std::vector<uint64_t> &sids, uint32_t shard_file, std::vector<NewSegs> &batches, Scratch &blobs, uint64_t *replaced_out) {
+ * `names` and whose segments `dir_runs` spliced from the shard and the files.  Fills batches[] and each span's new-segment range.
+ * A repeated time names its file, or the shard's rows when the file is `shard_file`.  Every batch's blob is followed by 1024
+ * readable bytes (k_append_gather reads past a page's end). */
+static int merge_spans(const SrcDir &dir, const std::vector<Run> &dir_runs, const std::vector<int32_t> &types, const std::vector<std::string> &names,
+                       const std::vector<Span *> &spans, const std::vector<uint64_t> &sids, uint32_t shard_file, std::vector<NewSegs> &batches,
+                       Scratch &blobs, uint64_t *replaced_out) {
     const uint32_t nc = dir.n_columns, ncol1 = nc + 1;
     int rc;
     /* scratch per row: decode (8 t + 4 file + 4 span + 9 per column), sort (4 + 4 perm, 8 keys), heads + scan (8), output slots
@@ -261,7 +265,8 @@ static int merge_spans(const SrcDir &dir, const std::vector<int32_t> &types, con
             if (he.code == M_STRING) { set_error("series sid %llu: string column \"%s\" has values in a span the merge re-encodes (there is no device string encoder)", sid, names[he.col].c_str()); return OG_E_UNSUPPORTED; }
             if (he.code == M_REPEAT && (uint32_t)he.file == shard_file) { set_error("series sid %llu: time %lld appears twice in the shard's rows inside a merged span", sid, he.time); return OG_E_CORRUPT; }
             if (he.code == M_REPEAT) { set_error("series sid %llu: time %lld appears twice in file %d inside a merged span", sid, he.time, he.file); return OG_E_CORRUPT; }
-            set_error("segment %d of the file set failed to decode (device code %d)", he.seg, he.code);
+            const Run &r = *std::prev(std::upper_bound(dir_runs.begin(), dir_runs.end(), (uint32_t)he.seg, [](uint32_t g, const Run &x) { return g < x.out0; }));
+            set_error("segment %u of the %s failed to decode (device code %d)", r.src0 + ((uint32_t)he.seg - r.out0), r.kind == SRC_SHARD ? "shard" : "file set", he.code);
             return he.code == D_UNSUPPORTED ? OG_E_UNSUPPORTED : OG_E_CORRUPT;
         }
         std::vector<uint32_t> h_out(nsp + 1), h_base(nsp);
@@ -473,8 +478,7 @@ static void sort_oldest_first(std::vector<uint32_t> &segs, const FileDir &fd, co
     std::stable_sort(segs.begin(), segs.end(), [&](uint32_t x, uint32_t y) { return rank(x) < rank(y); });
 }
 
-
-/* ---------------------------------------------------------------- og_shard_append_files */
+/* ---------------------------------------------------------------- the splice */
 
 /* one source of spliced segments: a device directory whose column c is column col[c] of the source (-1: the source lacks it) */
 struct SegSrc {
@@ -482,9 +486,6 @@ struct SegSrc {
     const uint32_t *seg_region; uint32_t region; /* data region of segment i: seg_region[i], or `region` when seg_region is null */
     const int32_t *col; uint32_t n_segments, n_columns;
 };
-enum { SRC_SHARD = 0, SRC_FILES = 1, SRC_MERGED = 2 };
-/* consecutive output segments [out0, next run's out0) of one series, from consecutive segments src0... of source `kind` */
-struct Run { uint32_t out0, src0, series, kind; };
 struct SpliceP {
     SegSrc src[3];
     const Run *runs; uint32_t n_runs, n_out, n_columns;
@@ -585,23 +586,21 @@ __global__ void k_append_stats(const uint8_t *data, const uint64_t *off, const u
 struct Spliced {
     uint32_t n = 0, n_columns = 0;
     uint64_t *off = nullptr; uint32_t *len = nullptr, *rows = nullptr, *series = nullptr; int64_t *tmin = nullptr, *tmax = nullptr;
-    uint8_t *data = nullptr; uint64_t data_len = 0;
+    uint8_t *data = nullptr; uint64_t data_len = 0; /* null: the pages are in the files' region, at the offsets they have there */
 };
-/* k_append_splice over `runs`, then every referenced page copied from `regions` into one new buffer (+1024 zero bytes).  The
- * directory arrays and the buffer are taken from `own`. */
+/* k_append_splice over `runs`, then, when a run reads another region than the files', every referenced page copied from `regions`
+ * into one new buffer (+1024 zero bytes).  The directory arrays and the buffer are taken from `own`. */
 static int splice_and_gather(const SegSrc src[3], const std::vector<Run> &runs, uint32_t n_out, uint32_t n_columns,
                              const std::vector<const uint8_t *> &regions, Scratch &own, Spliced &out) {
     int rc;
     const uint64_t n_pages = (uint64_t)(n_columns + 1) * n_out;
     out.n = n_out; out.n_columns = n_columns;
     Scratch tmp;
-    uint32_t *region; Run *d_runs; uint64_t *sizes; const uint8_t **d_regions;
+    uint32_t *region; Run *d_runs;
     if ((rc = own.get(&out.off, n_pages)) || (rc = own.get(&out.len, n_pages)) || (rc = own.get(&out.rows, n_out)) ||
         (rc = own.get(&out.series, n_out)) || (rc = own.get(&out.tmin, n_out)) || (rc = own.get(&out.tmax, n_out)) ||
-        (rc = tmp.get(&region, n_out)) || (rc = tmp.get(&d_runs, runs.size())) || (rc = tmp.get(&sizes, n_pages + 1)) ||
-        (rc = tmp.get(&d_regions, regions.size())))
+        (rc = tmp.get(&region, n_out)) || (rc = tmp.get(&d_runs, runs.size())))
         return rc;
-    CU(cudaMemcpy(d_regions, regions.data(), regions.size() * sizeof(void *), cudaMemcpyHostToDevice));
     if (n_out) {
         CU(cudaMemcpy(d_runs, runs.data(), runs.size() * sizeof(Run), cudaMemcpyHostToDevice));
         SpliceP p;
@@ -610,9 +609,12 @@ static int splice_and_gather(const SegSrc src[3], const std::vector<Run> &runs, 
         p.off = out.off; p.len = out.len; p.rows = out.rows; p.series = out.series; p.region = region; p.tmin = out.tmin; p.tmax = out.tmax;
         k_append_splice<<<(n_out + 127) / 128, 128>>>(p);
     }
+    /* every page already lies in the files' region at the offsets just spliced: keep that region rather than copy the pages */
+    if (std::all_of(runs.begin(), runs.end(), [](const Run &r) { return r.kind == SRC_FILES; })) { CU(cudaGetLastError()); return OG_OK; }
+    uint64_t *sizes, *dst_off; const uint8_t **d_regions;
+    if ((rc = tmp.get(&sizes, n_pages + 1)) || (rc = tmp.get(&dst_off, n_pages + 1)) || (rc = tmp.get(&d_regions, regions.size()))) return rc;
+    CU(cudaMemcpy(d_regions, regions.data(), regions.size() * sizeof(void *), cudaMemcpyHostToDevice));
     k_append_sizes<<<(unsigned)((n_pages + 1 + 255) / 256), 256>>>(out.len, n_pages, sizes);
-    uint64_t *dst_off;
-    if ((rc = tmp.get(&dst_off, n_pages + 1))) return rc;
     {
         size_t tb = 0; void *t = nullptr;
         CU(cub::DeviceScan::ExclusiveSum(nullptr, tb, sizes, dst_off, n_pages + 1));
@@ -632,149 +634,10 @@ static int splice_and_gather(const SegSrc src[3], const std::vector<Run> &runs, 
     return OG_OK;
 }
 
-} // namespace ogpu
+/* ---------------------------------------------------------------- files into a shard */
 
-using namespace ogpu;
-
-extern "C" {
-
-OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, og_shard **out) {
-    if (!files || !out || n_files == 0) { set_error("null argument or no files"); return OG_E_INVAL; }
-    *out = nullptr;
-    int rc = ensure_device(); if (rc) return rc;
-    int dev = 0; CU(cudaGetDevice(&dev));
-    /* ---- checks, schema union by name (sorted), series union by sid (ascending) ---- */
-    std::map<std::string, int32_t> schema;
-    std::map<uint64_t, uint32_t> series_of_sid;
-    if ((rc = scan_files(files, n_files, "og_shard_open_files", schema, series_of_sid))) return rc;
-    std::vector<std::string> names; std::vector<int32_t> types;
-    for (auto &kv : schema) { names.push_back(kv.first); types.push_back(kv.second); }
-    std::vector<uint64_t> sids;
-    for (auto &kv : series_of_sid) { kv.second = (uint32_t)sids.size(); sids.push_back(kv.first); }
-    const uint32_t nc = (uint32_t)names.size(), ncol1 = nc + 1, NSER = (uint32_t)sids.size();
-    /* ---- the source directory: every segment of every file, file by file, page offsets rebased into one buffer ---- */
-    FileDir fd;
-    if ((rc = build_file_dir(files, n_files, names, fd))) return rc;
-    const uint32_t NSRC = fd.n;
-    std::vector<uint64_t> &off = fd.off; std::vector<uint32_t> &len = fd.len;
-    const std::vector<int64_t> &tmin = fd.tmin, &tmax = fd.tmax;
-    const std::vector<uint32_t> &src_file = fd.src_file;
-    /* ---- per series: ordered segments in file order (no overlap across files), out-of-order segments, the span ---- */
-    std::vector<std::vector<uint32_t>> ordered(NSER), ooo(NSER);
-    og_merge_info info{}; info.n_files = n_files;
-    if ((rc = split_segments(files, n_files, file_flags, fd, series_of_sid, sids, ordered, ooo, info))) return rc;
-    /* layout of the output series: kept ordered segments before the span, the span, kept ones after it */
-    std::vector<Span> span_store; span_store.reserve(NSER);
-    std::vector<uint32_t> before(NSER), after_begin(NSER);
-    std::vector<int> span_of(NSER, -1);
-    for (uint32_t u = 0; u < NSER; u++) {
-        const auto &o = ordered[u];
-        if (ooo[u].empty()) { before[u] = after_begin[u] = (uint32_t)o.size(); continue; }
-        int64_t lo, hi;
-        span_hull(ooo[u], fd, &lo, &hi);
-        uint32_t a, b;
-        span_bounds(o, fd, lo, hi, &a, &b);
-        before[u] = a; after_begin[u] = b;
-        Span sp; sp.series = u;
-        sp.src.assign(o.begin() + a, o.begin() + b);
-        sp.src.insert(sp.src.end(), ooo[u].begin(), ooo[u].end());
-        sort_oldest_first(sp.src, fd, file_flags);
-        span_of[u] = (int)span_store.size();
-        span_store.push_back(std::move(sp));
-    }
-    /* ---- upload (one H2D per file), validate + transcode Snappy over the whole file set; the transcoded directory and the row
-       counts come back ---- */
-    std::unique_ptr<og_shard> src;
-    {
-        std::vector<uint32_t> rows;
-        if ((rc = upload_files(files, n_files, names, types, dev, fd, src, rows))) return rc;
-        for (auto &sp : span_store) {
-            for (uint32_t g : sp.src) { sp.rows += rows[g]; sp.src_file.push_back(src_file[g]); sp.src_rows.push_back(rows[g]); }
-            info.series_merged++;
-            info.segments_rewritten_in += sp.src.size();
-        }
-        for (uint32_t u = 0; u < NSER; u++) for (uint32_t g : ooo[u]) info.out_of_order_rows += rows[g];
-    }
-    /* ---- device merge ---- */
-    std::vector<NewSegs> batches;
-    Scratch blobs; /* the pages of every batch, until they are copied into the output data */
-    cudaEvent_t ev0, ev1;
-    CU(cudaEventCreate(&ev0)); CU(cudaEventCreate(&ev1));
-    struct FreeEv { cudaEvent_t a, b; ~FreeEv() { cudaEventDestroy(a); cudaEventDestroy(b); } } free_ev{ev0, ev1};
-    CU(cudaEventRecord(ev0, 0));
-    {
-        std::vector<Span *> sp;
-        for (auto &x : span_store) sp.push_back(&x);
-        uint64_t replaced = 0;
-        if ((rc = merge_spans(dir_of(src.get()), types, names, sp, sids, UINT32_MAX, batches, blobs, &replaced))) return rc;
-        info.rows_replaced = replaced;
-    }
-    /* ---- final data: the file set's bytes, then the new pages of every batch ---- */
-    uint64_t new_len = src->data_len;
-    for (auto &b : batches) { b.base = (new_len + 15) & ~15ull; new_len = b.base + b.bytes; }
-    std::unique_ptr<og_shard> s(new og_shard);
-    s->device = dev; s->n_series = NSER; s->n_columns = nc; s->col_types = types; s->col_names = names; s->sids = sids;
-    if (batches.empty()) { s->d_data = src->d_data; src->d_data = nullptr; s->data_len = src->data_len; }
-    else {
-        if ((rc = dalloc(&s->d_data, new_len + 1024))) return rc;
-        s->data_len = new_len;
-        CU(cudaMemset(s->d_data, 0, new_len + 1024));
-        CU(cudaMemcpy(s->d_data, src->d_data, src->data_len, cudaMemcpyDeviceToDevice));
-        for (auto &b : batches) if (b.bytes) CU(cudaMemcpy(s->d_data + b.base, b.blob, b.bytes, cudaMemcpyDeviceToDevice));
-    }
-    CU(cudaEventRecord(ev1, 0));
-    if (batches.empty()) { s->snappy_pages = src->snappy_pages; s->snappy_bytes_in = src->snappy_bytes_in; s->snappy_bytes_out = src->snappy_bytes_out; }
-    s->rows_merged = !batches.empty();
-    src.reset();
-    /* ---- the output directory ---- */
-    std::vector<uint32_t> o_ssb(NSER + 1, 0);
-    std::vector<uint64_t> o_off; std::vector<uint32_t> o_len; std::vector<int64_t> o_tmin, o_tmax;
-    struct Ref { int batch; uint32_t seg; }; /* batch < 0: source segment */
-    std::vector<Ref> refs;
-    for (uint32_t u = 0; u < NSER; u++) {
-        o_ssb[u] = (uint32_t)refs.size();
-        const auto &o = ordered[u];
-        for (uint32_t i = 0; i < before[u]; i++) refs.push_back({-1, o[i]});
-        if (span_of[u] >= 0) { const Span &sp = span_store[span_of[u]]; for (uint32_t g = 0; g < sp.n_new; g++) refs.push_back({(int)sp.batch, sp.first_new + g}); }
-        for (uint32_t i = after_begin[u]; i < o.size(); i++) refs.push_back({-1, o[i]});
-        info.segments_kept += before[u] + (o.size() - after_begin[u]);
-    }
-    const uint32_t NOUT = (uint32_t)refs.size();
-    o_ssb[NSER] = NOUT;
-    o_off.resize((size_t)ncol1 * NOUT); o_len.resize((size_t)ncol1 * NOUT); o_tmin.resize(NOUT); o_tmax.resize(NOUT);
-    for (uint32_t i = 0; i < NOUT; i++) {
-        const Ref r = refs[i];
-        for (uint32_t c = 0; c < ncol1; c++) {
-            if (r.batch < 0) { o_off[(size_t)c * NOUT + i] = off[(size_t)c * NSRC + r.seg]; o_len[(size_t)c * NOUT + i] = len[(size_t)c * NSRC + r.seg]; }
-            else {
-                const NewSegs &b = batches[r.batch];
-                const uint32_t l = b.len[(size_t)c * b.n + r.seg];
-                o_off[(size_t)c * NOUT + i] = l ? b.base + b.off[(size_t)c * b.n + r.seg] : 0; o_len[(size_t)c * NOUT + i] = l;
-            }
-        }
-        if (r.batch < 0) { o_tmin[i] = tmin[r.seg]; o_tmax[i] = tmax[r.seg]; }
-        else { o_tmin[i] = batches[r.batch].tmin[r.seg]; o_tmax[i] = batches[r.batch].tmax[r.seg]; }
-        info.segments_rewritten_out += r.batch >= 0;
-    }
-    s->n_segments = NOUT; s->h_series_seg_begin = o_ssb;
-    s->tmin = INT64_MAX; s->tmax = INT64_MIN;
-    for (uint32_t i = 0; i < NOUT; i++) { s->tmin = std::min(s->tmin, o_tmin[i]); s->tmax = std::max(s->tmax, o_tmax[i]); }
-    if ((rc = upload_dir(s.get(), o_ssb.data(), o_tmin.data(), o_tmax.data(), o_off.data(), o_len.data(), sids.data()))) return rc;
-    if ((rc = shard_finalize(s.get(), false))) return rc;
-    float ms = 0;
-    CU(cudaEventElapsedTime(&ms, ev0, ev1));
-    info.merge_ms = ms;
-    info.rows_after_merge = s->n_rows;
-    s->merge = info;
-    *out = s.release();
-    return OG_OK;
-}
-
-OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files) {
-    if (!s || !files || n_files == 0) { set_error("null argument or no files"); return OG_E_INVAL; }
-    std::lock_guard<std::mutex> lock(s->live->mu); /* og_query_create waits until the append is done */
-    if (s->live->n) { set_error("%u queries on this shard are still open: destroy them before appending files", s->live->n); return OG_E_STATE; }
-    CU(cudaSetDevice(s->device));
+/* the files join `s`: og_shard_append_files, and og_shard_open_files on an empty shard.  `who` names the caller in refusals. */
+static int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, const char *who) {
     int rc;
     /* ---- checks; schema union with the shard's columns (sorted by name), series union with its sids (ascending) ---- */
     const uint32_t onc = s->n_columns, ONSER = s->n_series, ONSEG = s->n_segments;
@@ -782,7 +645,7 @@ OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const 
     for (uint32_t c = 0; c < onc; c++) schema[s->col_names[c]] = s->col_types[c];
     if (schema.size() != onc) { set_error("the shard holds two columns of one name"); return OG_E_UNSUPPORTED; }
     std::map<uint64_t, uint32_t> series_of_sid;
-    if ((rc = scan_files(files, n_files, "og_shard_append_files", schema, series_of_sid))) return rc;
+    if ((rc = scan_files(files, n_files, who, schema, series_of_sid))) return rc;
     std::map<uint64_t, uint32_t> old_of_sid;
     for (uint32_t i = 0; i < ONSER; i++) {
         if (!old_of_sid.emplace(s->sids[i], i).second) { set_error("the shard holds sid %llu twice", (unsigned long long)s->sids[i]); return OG_E_UNSUPPORTED; }
@@ -884,8 +747,8 @@ OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const 
     CU(cudaEventCreate(&ev0)); CU(cudaEventCreate(&ev1));
     struct FreeEv { cudaEvent_t a, b; ~FreeEv() { cudaEventDestroy(a); cudaEventDestroy(b); } } free_ev{ev0, ev1};
     CU(cudaEventRecord(ev0, 0));
-    /* ---- merge: the spans' source pages gathered into one buffer (the shard's rows first, then the new files in sequence,
-       ordered before out-of-order), then merge_spans as at open ---- */
+    /* ---- merge: the spans' source segments spliced into one directory (the shard's rows first, then the new files in sequence,
+       ordered before out-of-order), then merge_spans ---- */
     std::vector<NewSegs> batches;
     Scratch blobs, msrc_own;
     if (!span_store.empty()) {
@@ -921,11 +784,11 @@ OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const 
                 for (uint32_t i : sp.src) { sp.src_rows.push_back(rows[i]); sp.rows += rows[i]; }
         }
         SrcDir dir;
-        dir.data = ms.data; dir.page_off = ms.off; dir.page_len = ms.len; dir.seg_rows = ms.rows; dir.n_segments = ms.n; dir.n_columns = nc;
+        dir.data = ms.data ? ms.data : nw->d_data; dir.page_off = ms.off; dir.page_len = ms.len; dir.seg_rows = ms.rows; dir.n_segments = ms.n; dir.n_columns = nc;
         std::vector<Span *> sp;
         for (auto &x : span_store) sp.push_back(&x);
         uint64_t replaced = 0;
-        if ((rc = merge_spans(dir, types, names, sp, sids, n_files, batches, blobs, &replaced))) return rc;
+        if ((rc = merge_spans(dir, runs, types, names, sp, sids, n_files, batches, blobs, &replaced))) return rc;
         info.rows_replaced = replaced;
     }
     /* ---- the merged segments as one source directory, each batch's blob its own region ---- */
@@ -982,11 +845,12 @@ OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const 
         emit(u, after_begin[u], total);
     }
     o_ssb[NSER] = NOUT;
-    /* ---- gather the live pages into the new data region ---- */
+    /* ---- the new directory, and the live pages gathered into a new data region or left in the files' one ---- */
     std::unique_ptr<og_shard> out(new og_shard);
     Scratch out_own;
     Spliced sd;
     if ((rc = splice_and_gather(src, runs, NOUT, nc, regions, out_own, sd))) return rc;
+    if (!sd.data) { sd.data = nw->d_data; sd.data_len = nw->data_len; nw->d_data = nullptr; out_own.bufs.push_back(sd.data); }
     CU(cudaEventRecord(ev1, 0));
     /* ---- derived state ---- */
     {
@@ -1006,7 +870,7 @@ OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const 
         if (err[0]) { set_error("segment %d: time page failed to parse after the append (device code %d)", err[1], err[0]); return OG_E_CORRUPT; }
         out->n_rows = tot[0]; out->page_bytes = tot[1]; out->irregular_time_pages = tot[2]; out->tmin = range[0]; out->tmax = range[1];
     }
-    /* the Snappy counters follow og_shard_open_files over the whole set: a merge there drops them */
+    /* the Snappy counters hold while every transcoded page is in the shard: the first merge drops them */
     out->rows_merged = s->rows_merged || !batches.empty();
     if (!out->rows_merged) {
         out->snappy_pages = s->snappy_pages + nw->snappy_pages;
@@ -1037,6 +901,32 @@ OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const 
         s->il.assign(s->n_columns, og_shard::IlCol{});
     }
     return OG_OK;
+}
+
+} // namespace ogpu
+
+using namespace ogpu;
+
+extern "C" {
+
+OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, og_shard **out) {
+    if (!files || !out || n_files == 0) { set_error("null argument or no files"); return OG_E_INVAL; }
+    *out = nullptr;
+    int rc = ensure_device(); if (rc) return rc;
+    std::unique_ptr<og_shard> s(new og_shard); /* an open is an append to an empty shard */
+    CU(cudaGetDevice(&s->device));
+    s->h_series_seg_begin = {0};
+    if ((rc = add_files(s.get(), files, file_flags, n_files, "og_shard_open_files"))) return rc;
+    *out = s.release();
+    return OG_OK;
+}
+
+OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files) {
+    if (!s || !files || n_files == 0) { set_error("null argument or no files"); return OG_E_INVAL; }
+    std::lock_guard<std::mutex> lock(s->live->mu); /* og_query_create waits until the append is done */
+    if (s->live->n) { set_error("%u queries on this shard are still open: destroy them before appending files", s->live->n); return OG_E_STATE; }
+    CU(cudaSetDevice(s->device));
+    return add_files(s, files, file_flags, n_files, "og_shard_append_files");
 }
 
 OG_API int og_shard_merge_info(const og_shard *s, og_merge_info *out) {

@@ -241,6 +241,7 @@ def test_out_of_order_flushes_equal_the_fresh_open(seg_rows):
         assert mi["segments_kept"] + mi["segments_rewritten_out"] == ex["seg_tmin"].size
         # the data region holds the live pages only: the pages this call rewrote are left behind
         assert _data_excess(sh) == 0
+        assert _data_excess(fresh) == 0
         _all_paths(sh, files, seg_rows)
         fresh.close()
     sh.close()

@@ -275,23 +275,28 @@ def test_preagg_cells_equal_the_oracle_per_series_aggregates():
 
 
 # ---------------------------------------------------------------- 5: merged and downsampled shards
-def test_merged_shard_writes_without_its_dead_pages():
+def test_merged_shard_writes_its_live_pages():
     cols = [("u", "f_hi", 0), ("v", "i_s8b", 0.05)]
     ordered = make_chunks(31, 5, cols, lambda rng, s: [1000, 1000, 400], t0=T0)
     late = make_chunks(32, 5, cols, lambda rng, s: [300], ("s8b",), t0=T0 + 500 * SEC)   # rows inside the first ordered segments
     merged = Shard.open_files([(M.build(ordered, b"m"), False), (M.build(late, b"m"), True)])
+    ordered_only = Shard.open_files([(M.build(ordered, b"m"), False)])
     back = None
     try:
+        # without a merge the shard keeps the file's region, CRCs and metadata included: the writer takes only the pages from it
+        eo = ordered_only.export()
+        referenced_o = int(eo["page_len"].sum())
+        assert referenced_o < eo["data"].size
+        assert M.parse(write_tssp(ordered_only, "m"))["trailer"]["data_size"] == referenced_o + 4 * 3 * 5
         mi = merged.merge_info()
         assert mi["series_merged"] == 5 and mi["segments_rewritten_in"] > 0
         f = write_tssp(merged, "m")
         _check_crcs(f)
         ex = merged.export()
         referenced = int(ex["page_len"].sum())
-        assert referenced < ex["data"].size, "the merged shard keeps the rewritten source pages"
+        assert referenced == ex["data"].size, "the merged shard holds only the pages its directory references"
         p = M.parse(f)
         assert p["trailer"]["data_size"] == referenced + 4 * 3 * 5        # only referenced pages, plus one CRC per column of a chunk
-        assert len(f) < ex["data"].size
         back = Shard.open_tssp(f)
         assert _referenced_pages(ex) == _referenced_pages(back.export())
         assert _same_answers(merged, back, [L.TYPE_FLOAT, L.TYPE_INT], filter_col=1) > 10
@@ -303,6 +308,7 @@ def test_merged_shard_writes_without_its_dead_pages():
         assert sum(struct.unpack(">I", ch["columns"][2]["preagg"])[0] for ch in p["chunks"]) == mi["rows_after_merge"] == info["n_rows"]
     finally:
         merged.close()
+        ordered_only.close()
         if back:
             back.close()
 
