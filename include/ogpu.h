@@ -318,6 +318,41 @@ OG_API int og_shard_merge_info(const og_shard *s, og_merge_info *out); /* og_sha
  *   (OG_SHARD_DEVICE_DATA) gets its own buffer; the caller's buffer is never written. */
 OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files);
 
+/* ---- compaction of an open shard (csrc/compact.cu).  Replaces the device pass of the reference's non-streaming level
+ * compaction (engine/immutable/compact.go:175-242): a series' merged records written through MsBuilder.WriteRecord -> WriteData
+ * (msbuilder.go:1151), which cuts them into segments of R rows from the start of the series, every column of the chunk schema
+ * (stream_compact.go:303 mergeSchema) with a page in every segment, null rows where a source lacked the column
+ * (stream_compact.go:833-840 newNilCol).
+ * A series is compact when every segment but its last holds R rows, its last 1..R, and every column has a page (an all-null page
+ * counts) in every segment of the series or in none.  After the call every series is compact:
+ *   a compact series keeps its directory entries and page bytes; a series with a column in only some segments is re-cut from
+ *   its first segment; any other series is re-cut from its first segment that is not its last and holds fewer than R rows, or
+ *   holds more than R rows (the segments before it end at multiples of R and keep their bytes).  Re-cut rows go into
+ *   ceil(rows / R) new segments, every column of the series with a page in each (null where a source segment lacked it), pages
+ *   from the encoders of og_encode_pages (raw page for a float segment Gorilla refuses), seg_tmin / seg_tmax from the rows.
+ *   Rows, og_shard_info's n_rows / tmin / tmax and og_shard_merge_info are unchanged; n_segments and page_bytes are recomputed.
+ *   An already compact shard is left untouched (no copy, every counter 0).
+ * Refused, the shard left as it was (only its interleaved copies may have been dropped; rebuilt on first use):
+ *   rows_per_segment above 1000 or non-zero flags (OG_E_INVAL); a string value inside a re-cut range (OG_E_UNSUPPORTED, naming
+ *   the sid and the column: there is no device string encoder); a time that does not strictly ascend inside a re-cut range
+ *   (OG_E_CORRUPT, naming the sid and the time); a live og_query of the shard (OG_E_STATE; og_query_create on another thread
+ *   waits while a compaction runs).
+ *   Cost: the re-cut rows are decoded into segment slots and encoded in batches under a device-memory budget, then the live pages
+ *   are gathered into a new data region.  Peak device memory: about the live pages twice, plus one batch's scratch. */
+typedef struct og_compact_desc {
+    uint32_t rows_per_segment; /* R; 0 = 1000 (lib/util/util.go:72); 1..1000 (og_encode_pages' range); else OG_E_INVAL */
+    uint32_t flags;            /* 0; anything else OG_E_INVAL */
+} og_compact_desc;
+typedef struct og_compact_info {
+    uint64_t series_rewritten;                        /* series with at least one re-cut segment */
+    uint64_t segments_kept;                           /* segments carried over byte for byte (0 when nothing was re-cut) */
+    uint64_t segments_rewritten_in, segments_rewritten_out;
+    uint64_t rows_rewritten;
+    double compact_ms;                                /* CUDA events around the device pass, from the first decode to the gather
+                                                         of the live pages (as og_merge_info.merge_ms) */
+} og_compact_info;
+OG_API int og_shard_compact(og_shard *s, const og_compact_desc *d, og_compact_info *info /* may be NULL */);
+
 /* ---- query (aggregate cursor tree) ---- */
 /* OG_E_UNSUPPORTED when the first or last row in range lies in a window that Window() clamps at the int64 time limits
  * (DESIGN.md "Deviations") */

@@ -112,6 +112,15 @@ class MergeInfo(C.Structure):
                 ("merge_ms", C.c_double)]
 
 
+class CompactDesc(C.Structure):
+    _fields_ = [("rows_per_segment", C.c_uint32), ("flags", C.c_uint32)]
+
+
+class CompactInfo(C.Structure):
+    _fields_ = [("series_rewritten", C.c_uint64), ("segments_kept", C.c_uint64), ("segments_rewritten_in", C.c_uint64),
+                ("segments_rewritten_out", C.c_uint64), ("rows_rewritten", C.c_uint64), ("compact_ms", C.c_double)]
+
+
 class TsspWriteDesc(C.Structure):
     _fields_ = [("measurement", C.c_char_p), ("series_begin", C.c_uint32), ("series_end", C.c_uint32), ("flags", C.c_uint32)]
 
@@ -126,7 +135,7 @@ EXPORTS = [
     "og_downsample", "og_downsampled_desc", "og_downsampled_export", "og_downsampled_free",
     "og_downsample_shard", "og_downsampled_timing",
     "og_tssp_parse", "og_tssp_desc", "og_tssp_measurement", "og_tssp_time_range", "og_tssp_free",
-    "og_shard_open_files", "og_shard_merge_info", "og_shard_append_files",
+    "og_shard_open_files", "og_shard_merge_info", "og_shard_append_files", "og_shard_compact",
     "og_shard_write_tssp", "og_tssp_image_size", "og_tssp_image_export", "og_tssp_image_timing", "og_tssp_image_free",
 ]
 
@@ -158,6 +167,7 @@ def lib():
     L.og_shard_open_files.argtypes = [C.POINTER(ShardDesc), u32p, C.c_uint32, C.POINTER(C.c_void_p)]
     L.og_shard_merge_info.argtypes = [C.c_void_p, C.POINTER(MergeInfo)]
     L.og_shard_append_files.argtypes = [C.c_void_p, C.POINTER(ShardDesc), u32p, C.c_uint32]
+    L.og_shard_compact.argtypes = [C.c_void_p, C.POINTER(CompactDesc), C.POINTER(CompactInfo)]
     L.og_shard_close.argtypes = [C.c_void_p]
     L.og_shard_close.restype = None
     L.og_shard_info.argtypes = [C.c_void_p, u64p, u64p, u64p, u64p, i64p, i64p]

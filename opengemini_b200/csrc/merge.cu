@@ -47,6 +47,7 @@
 
 #include "decode.cuh"
 #include "internal.h"
+#include "span_pass.h"
 
 namespace ogpu {
 
@@ -59,16 +60,6 @@ int encode_pages(int32_t type, int32_t is_time, const void *d_values, const uint
                  bool nan_raw); /* encode.cu */
 
 #define MERGE_RPS 1000u           /* rows per rewritten segment: lib/util/util.go:72 */
-#define MERGE_PAGE_BOUND 8704u    /* largest page the encoders write for 1000 rows (encode.cu PAGE_STRIDE) */
-
-/* the part of the device directory the merge reads */
-struct SrcDir {
-    const uint8_t *data; const uint64_t *page_off; const uint32_t *page_len; const uint32_t *seg_rows;
-    uint32_t n_segments, n_columns;
-};
-
-enum { M_STRING = 100, M_REPEAT = 101 };
-struct MergeErr { int code, seg, col, span, file; long long time; };
 
 __device__ __forceinline__ bool merge_claim(MergeErr *e, int code) { return atomicCAS(&e->code, 0, code) == 0; }
 
@@ -163,10 +154,6 @@ __global__ void k_merge_combine(const int64_t *t, const uint32_t *perm, const ui
     if (slot == MERGE_RPS - 1 || local == cnt - 1) seg_tmax[g] = tt;
 }
 
-enum { SRC_SHARD = 0, SRC_FILES = 1, SRC_MERGED = 2 };
-/* consecutive output segments [out0, next run's out0) of one series, from consecutive segments src0... of source `kind` */
-struct Run { uint32_t out0, src0, series, kind; };
-
 /* a rewritten span: source segments (file order) -> new segments */
 struct Span {
     uint32_t series;                 /* union series index */
@@ -174,13 +161,6 @@ struct Span {
     std::vector<uint32_t> src_file, src_rows; /* per source segment: its file (one file never repeats a time) and its rows */
     uint64_t rows = 0;
     uint32_t batch = 0, first_new = 0, n_new = 0; /* new segments [first_new, first_new + n_new) of batch `batch` */
-};
-struct NewSegs { /* what one batch produced, on the host */
-    std::vector<uint64_t> off; std::vector<uint32_t> len; /* [(n_cols+1) * n] relative to the batch blob */
-    std::vector<int64_t> tmin, tmax;
-    std::vector<uint32_t> rows;
-    uint8_t *blob = nullptr; uint64_t bytes = 0;
-    uint32_t n = 0;
 };
 
 /* Merge every span on the device, batch by batch: the spans' source segments are read through `dir`, whose columns are `types` /
@@ -196,13 +176,7 @@ static int merge_spans(const SrcDir &dir, const std::vector<Run> &dir_runs, cons
        (8 + 9 per column), encoder staging and blob (2 x 8704 / 1000 per page) */
     const uint64_t per_row = 48 + 18ull * nc + 2ull * ncol1 * MERGE_PAGE_BOUND / MERGE_RPS + 64;
     uint64_t cap_rows;
-    {
-        size_t fr = 0, tot = 0;
-        CU(dev_mem_info(&fr, &tot));
-        cap_rows = std::max<uint64_t>(MERGE_RPS, (uint64_t)(fr / 4) / per_row);
-        if (const char *ov = getenv("OGPU_MERGE_BATCH_ROWS")) cap_rows = std::max<uint64_t>(1, strtoull(ov, nullptr, 10)); /* test hook */
-        cap_rows = std::min<uint64_t>(cap_rows, 1ull << 30);
-    }
+    if ((rc = batch_cap_rows(per_row, MERGE_RPS, "OGPU_MERGE_BATCH_ROWS", &cap_rows))) return rc;
     std::vector<int64_t> h_zero;
     unsigned long long *d_rep; MergeErr *d_err; int32_t *d_types;
     Scratch keep;
@@ -262,12 +236,11 @@ static int merge_spans(const SrcDir &dir, const std::vector<Run> &dir_runs, cons
         CU(cudaMemcpy(&he, d_err, sizeof he, cudaMemcpyDeviceToHost));
         if (he.code) {
             const unsigned long long sid = (unsigned long long)sids[spans[sp0 + he.span]->series];
-            if (he.code == M_STRING) { set_error("series sid %llu: string column \"%s\" has values in a span the merge re-encodes (there is no device string encoder)", sid, names[he.col].c_str()); return OG_E_UNSUPPORTED; }
+            if (he.code == M_STRING) return string_refusal(sid, names[he.col], "the merge");
             if (he.code == M_REPEAT && (uint32_t)he.file == shard_file) { set_error("series sid %llu: time %lld appears twice in the shard's rows inside a merged span", sid, he.time); return OG_E_CORRUPT; }
             if (he.code == M_REPEAT) { set_error("series sid %llu: time %lld appears twice in file %d inside a merged span", sid, he.time, he.file); return OG_E_CORRUPT; }
             const Run &r = *std::prev(std::upper_bound(dir_runs.begin(), dir_runs.end(), (uint32_t)he.seg, [](uint32_t g, const Run &x) { return g < x.out0; }));
-            set_error("segment %u of the %s failed to decode (device code %d)", r.src0 + ((uint32_t)he.seg - r.out0), r.kind == SRC_SHARD ? "shard" : "file set", he.code);
-            return he.code == D_UNSUPPORTED ? OG_E_UNSUPPORTED : OG_E_CORRUPT;
+            return decode_failure(he.code, r.src0 + ((uint32_t)he.seg - r.out0), r.kind == SRC_SHARD ? "shard" : "file set");
         }
         std::vector<uint32_t> h_out(nsp + 1), h_base(nsp);
         CU(cudaMemcpy(h_out.data(), out_begin, (nsp + 1) * 4ull, cudaMemcpyDeviceToHost));
@@ -297,33 +270,16 @@ static int merge_spans(const SrcDir &dir, const std::vector<Run> &dir_runs, cons
                                                    out_t, d_cols, out_ok, out_rows, d_tmin, d_tmax, d_rep);
         CU(cudaGetLastError());
         /* encode every column (string columns: no values inside a span, so no page) */
-        uint8_t *blob; uint64_t *d_off; uint32_t *d_len;
+        uint8_t *blob;
         const uint64_t cap = (uint64_t)NS * ncol1 * MERGE_PAGE_BOUND;
-        if ((rc = b.get(&blob, cap)) || (rc = b.get(&d_off, (size_t)ncol1 * NS)) || (rc = b.get(&d_len, (size_t)ncol1 * NS))) return rc;
-        CU(cudaMemset(d_len, 0, (size_t)ncol1 * NS * 4)); CU(cudaMemset(d_off, 0, (size_t)ncol1 * NS * 8));
+        if ((rc = b.get(&blob, cap))) return rc;
         uint64_t used = 0;
-        ns.off.assign((size_t)ncol1 * NS, 0); ns.len.assign((size_t)ncol1 * NS, 0);
-        for (uint32_t c = 0; c <= nc; c++) {
-            const bool is_time = c == nc;
-            if (!is_time && types[c] == OG_TYPE_STRING) continue;
-            uint64_t tot = 0;
-            rc = encode_pages(is_time ? OG_TYPE_INT : types[c], is_time ? 1 : 0, is_time ? (const void *)out_t : (const void *)h_cols[c],
-                              is_time ? nullptr : out_ok + (size_t)c * out_rows, d_rows, NS, MERGE_RPS, blob + used, cap - used,
-                              d_off + (size_t)c * NS, d_len + (size_t)c * NS, &tot, true);
-            if (rc) return rc;
-            CU(cudaMemcpy(ns.off.data() + (size_t)c * NS, d_off + (size_t)c * NS, NS * 8ull, cudaMemcpyDeviceToHost));
-            CU(cudaMemcpy(ns.len.data() + (size_t)c * NS, d_len + (size_t)c * NS, NS * 4ull, cudaMemcpyDeviceToHost));
-            for (uint32_t g = 0; g < NS; g++) ns.off[(size_t)c * NS + g] += used;
-            used += tot;
-        }
+        if ((rc = encode_columns(types, out_t, h_cols, out_ok, out_rows, d_rows, NS, MERGE_RPS, blob, cap, ns, &used))) return rc;
         ns.tmin.resize(NS); ns.tmax.resize(NS); ns.rows = h_rows;
         CU(cudaMemcpy(ns.tmin.data(), d_tmin, NS * 8ull, cudaMemcpyDeviceToHost));
         CU(cudaMemcpy(ns.tmax.data(), d_tmax, NS * 8ull, cudaMemcpyDeviceToHost));
         /* keep only the bytes written: the batch's scratch goes back to the pool before the next batch */
-        if ((rc = blobs.get(&ns.blob, used + 1024))) return rc;
-        CU(cudaMemcpy(ns.blob, blob, used, cudaMemcpyDeviceToDevice));
-        CU(cudaMemset(ns.blob + used, 0, 1024));
-        ns.bytes = used;
+        if ((rc = keep_blob(blob, used, blobs, ns))) return rc;
         batches.push_back(std::move(ns));
         sp0 = sp1;
     }
@@ -480,12 +436,6 @@ static void sort_oldest_first(std::vector<uint32_t> &segs, const FileDir &fd, co
 
 /* ---------------------------------------------------------------- the splice */
 
-/* one source of spliced segments: a device directory whose column c is column col[c] of the source (-1: the source lacks it) */
-struct SegSrc {
-    const uint64_t *off; const uint32_t *len, *rows; const int64_t *tmin, *tmax;
-    const uint32_t *seg_region; uint32_t region; /* data region of segment i: seg_region[i], or `region` when seg_region is null */
-    const int32_t *col; uint32_t n_segments, n_columns;
-};
 struct SpliceP {
     SegSrc src[3];
     const Run *runs; uint32_t n_runs, n_out, n_columns;
@@ -582,15 +532,9 @@ __global__ void k_append_stats(const uint8_t *data, const uint64_t *off, const u
     atomicMax(&range[1], (long long)tmax[g]);
 }
 
-/* a spliced directory and the data region its pages were gathered into */
-struct Spliced {
-    uint32_t n = 0, n_columns = 0;
-    uint64_t *off = nullptr; uint32_t *len = nullptr, *rows = nullptr, *series = nullptr; int64_t *tmin = nullptr, *tmax = nullptr;
-    uint8_t *data = nullptr; uint64_t data_len = 0; /* null: the pages are in the files' region, at the offsets they have there */
-};
 /* k_append_splice over `runs`, then, when a run reads another region than the files', every referenced page copied from `regions`
  * into one new buffer (+1024 zero bytes).  The directory arrays and the buffer are taken from `own`. */
-static int splice_and_gather(const SegSrc src[3], const std::vector<Run> &runs, uint32_t n_out, uint32_t n_columns,
+int splice_and_gather(const SegSrc src[3], const std::vector<Run> &runs, uint32_t n_out, uint32_t n_columns,
                              const std::vector<const uint8_t *> &regions, Scratch &own, Spliced &out) {
     int rc;
     const uint64_t n_pages = (uint64_t)(n_columns + 1) * n_out;
@@ -632,6 +576,120 @@ static int splice_and_gather(const SegSrc src[3], const std::vector<Run> &runs, 
     CU(cudaMemcpy(out.off, dst_off, n_pages * 8, cudaMemcpyDeviceToDevice));
     CU(cudaDeviceSynchronize()); /* tmp goes back to the pool */
     return OG_OK;
+}
+
+/* ---------------------------------------------------------------- shared with compaction (span_pass.h) */
+
+int batch_cap_rows(uint64_t per_row, uint64_t floor_rows, const char *env, uint64_t *cap) {
+    size_t fr = 0, tot = 0;
+    CU(dev_mem_info(&fr, &tot));
+    *cap = std::max<uint64_t>(floor_rows, (uint64_t)(fr / 4) / per_row);
+    if (const char *ov = getenv(env)) *cap = std::max<uint64_t>(1, strtoull(ov, nullptr, 10)); /* test hook */
+    *cap = std::min<uint64_t>(*cap, 1ull << 30);
+    return OG_OK;
+}
+
+int encode_columns(const std::vector<int32_t> &types, const int64_t *d_times, const std::vector<uint8_t *> &d_cols, const uint8_t *d_ok,
+                   size_t out_rows, const uint32_t *d_rows, uint32_t n, uint32_t rps, uint8_t *blob, uint64_t cap, NewSegs &ns, uint64_t *used) {
+    int rc;
+    const uint32_t nc = (uint32_t)types.size(), ncol1 = nc + 1;
+    Scratch t;
+    uint64_t *d_off; uint32_t *d_len;
+    if ((rc = t.get(&d_off, (size_t)ncol1 * n)) || (rc = t.get(&d_len, (size_t)ncol1 * n))) return rc;
+    CU(cudaMemset(d_len, 0, (size_t)ncol1 * n * 4)); CU(cudaMemset(d_off, 0, (size_t)ncol1 * n * 8));
+    ns.off.assign((size_t)ncol1 * n, 0); ns.len.assign((size_t)ncol1 * n, 0);
+    for (uint32_t c = 0; c <= nc; c++) {
+        const bool is_time = c == nc;
+        if (!is_time && types[c] == OG_TYPE_STRING) continue;
+        uint64_t tot = 0;
+        rc = encode_pages(is_time ? OG_TYPE_INT : types[c], is_time ? 1 : 0, is_time ? (const void *)d_times : (const void *)d_cols[c],
+                          is_time ? nullptr : d_ok + (size_t)c * out_rows, d_rows, n, rps, blob + *used, cap - *used,
+                          d_off + (size_t)c * n, d_len + (size_t)c * n, &tot, true);
+        if (rc) return rc;
+        CU(cudaMemcpy(ns.off.data() + (size_t)c * n, d_off + (size_t)c * n, n * 8ull, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(ns.len.data() + (size_t)c * n, d_len + (size_t)c * n, n * 4ull, cudaMemcpyDeviceToHost));
+        for (uint32_t g = 0; g < n; g++) ns.off[(size_t)c * n + g] += *used;
+        *used += tot;
+    }
+    return OG_OK;
+}
+
+int keep_blob(const uint8_t *blob, uint64_t used, Scratch &blobs, NewSegs &ns) {
+    int rc;
+    if ((rc = blobs.get(&ns.blob, used + 1024))) return rc;
+    if (used) CU(cudaMemcpy(ns.blob, blob, used, cudaMemcpyDeviceToDevice));
+    CU(cudaMemset(ns.blob + used, 0, 1024));
+    ns.bytes = used;
+    return OG_OK;
+}
+
+int string_refusal(unsigned long long sid, const std::string &column, const char *pass) {
+    set_error("series sid %llu: string column \"%s\" has values in a span %s re-encodes (there is no device string encoder)", sid, column.c_str(), pass);
+    return OG_E_UNSUPPORTED;
+}
+
+int decode_failure(int device_code, uint32_t seg, const char *where) {
+    set_error("segment %u of the %s failed to decode (device code %d)", seg, where, device_code);
+    return device_code == D_UNSUPPORTED ? OG_E_UNSUPPORTED : OG_E_CORRUPT;
+}
+
+int batches_source(const std::vector<NewSegs> &batches, uint32_t nc, const int32_t *d_identity, uint32_t first_region,
+                   std::vector<const uint8_t *> &regions, Scratch &own, SegSrc &out, std::vector<uint32_t> &m_first) {
+    int rc;
+    m_first.assign(batches.size() + 1, 0);
+    for (size_t b = 0; b < batches.size(); b++) m_first[b + 1] = m_first[b] + batches[b].n;
+    const uint32_t NM = m_first[batches.size()];
+    if (!NM) return OG_OK;
+    std::vector<uint64_t> off((size_t)(nc + 1) * NM); std::vector<uint32_t> len((size_t)(nc + 1) * NM), rows(NM), reg(NM);
+    std::vector<int64_t> tmin(NM), tmax(NM);
+    for (size_t b = 0; b < batches.size(); b++) {
+        const NewSegs &B = batches[b];
+        regions.push_back(B.blob);
+        for (uint32_t g = 0; g < B.n; g++) {
+            const uint32_t m = m_first[b] + g;
+            for (uint32_t c = 0; c <= nc; c++) { off[(size_t)c * NM + m] = B.off[(size_t)c * B.n + g]; len[(size_t)c * NM + m] = B.len[(size_t)c * B.n + g]; }
+            rows[m] = B.rows[g]; reg[m] = first_region + (uint32_t)b; tmin[m] = B.tmin[g]; tmax[m] = B.tmax[g];
+        }
+    }
+    uint64_t *d_off; uint32_t *d_len, *d_rows, *d_reg; int64_t *d_tmin, *d_tmax;
+    if ((rc = own.get(&d_off, off.size())) || (rc = own.get(&d_len, len.size())) || (rc = own.get(&d_rows, NM)) || (rc = own.get(&d_reg, NM)) ||
+        (rc = own.get(&d_tmin, NM)) || (rc = own.get(&d_tmax, NM)))
+        return rc;
+    CU(cudaMemcpy(d_off, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_len, len.data(), len.size() * 4, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_rows, rows.data(), NM * 4ull, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_reg, reg.data(), NM * 4ull, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_tmin, tmin.data(), NM * 8ull, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_tmax, tmax.data(), NM * 8ull, cudaMemcpyHostToDevice));
+    out = SegSrc{d_off, d_len, d_rows, d_tmin, d_tmax, d_reg, 0, d_identity, NM, nc};
+    return OG_OK;
+}
+
+int spliced_totals(const Spliced &sd, uint32_t nc, ShardState &out, const char *who) {
+    int rc;
+    Scratch t;
+    unsigned long long *d_tot; uint32_t *d_max; long long *d_range; int *d_err;
+    if ((rc = t.get(&d_tot, 3)) || (rc = t.get(&d_max, 1)) || (rc = t.get(&d_range, 2)) || (rc = t.get(&d_err, 2))) return rc;
+    const long long r0[2] = {INT64_MAX, INT64_MIN};
+    CU(cudaMemset(d_tot, 0, 24)); CU(cudaMemset(d_max, 0, 4)); CU(cudaMemset(d_err, 0, 8));
+    CU(cudaMemcpy(d_range, r0, 16, cudaMemcpyHostToDevice));
+    if (sd.n) k_append_stats<<<(sd.n + 127) / 128, 128>>>(sd.data, sd.off, sd.len, sd.rows, sd.tmin, sd.tmax, sd.n, nc, d_tot, d_max, d_range, d_err);
+    CU(cudaGetLastError());
+    unsigned long long tot[3]; long long range[2]; int err[2];
+    CU(cudaMemcpy(tot, d_tot, 24, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(&out.max_seg_rows, d_max, 4, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(range, d_range, 16, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(err, d_err, 8, cudaMemcpyDeviceToHost));
+    if (err[0]) { set_error("segment %d: time page failed to parse after %s (device code %d)", err[1], who, err[0]); return OG_E_CORRUPT; }
+    out.n_rows = tot[0]; out.page_bytes = tot[1]; out.irregular_time_pages = tot[2]; out.tmin = range[0]; out.tmax = range[1];
+    return OG_OK;
+}
+
+void take_spliced(Scratch &own, Spliced &sd, ShardState &out) {
+    auto take = [&](void *p) { own.bufs.erase(std::find(own.bufs.begin(), own.bufs.end(), p)); };
+    for (void *p : {(void *)sd.off, (void *)sd.len, (void *)sd.rows, (void *)sd.series, (void *)sd.tmin, (void *)sd.tmax, (void *)sd.data}) take(p);
+    out.d_page_off = sd.off; out.d_page_len = sd.len; out.d_seg_rows = sd.rows; out.d_seg_series = sd.series; out.d_tmin = sd.tmin; out.d_tmax = sd.tmax;
+    out.d_data = sd.data; out.data_len = sd.data_len; out.owns_data = true;
 }
 
 /* ---------------------------------------------------------------- files into a shard */
@@ -792,36 +850,10 @@ static int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *fi
         info.rows_replaced = replaced;
     }
     /* ---- the merged segments as one source directory, each batch's blob its own region ---- */
-    std::vector<uint32_t> m_first(batches.size() + 1, 0);
-    for (size_t b = 0; b < batches.size(); b++) m_first[b + 1] = m_first[b] + batches[b].n;
-    const uint32_t NM = m_first[batches.size()];
+    std::vector<uint32_t> m_first;
     std::vector<const uint8_t *> regions = {s->d_data, nw->d_data};
     Scratch m_own;
-    if (NM) {
-        std::vector<uint64_t> off((size_t)(nc + 1) * NM); std::vector<uint32_t> len((size_t)(nc + 1) * NM), rows(NM), reg(NM);
-        std::vector<int64_t> tmin(NM), tmax(NM);
-        for (size_t b = 0; b < batches.size(); b++) {
-            const NewSegs &B = batches[b];
-            regions.push_back(B.blob);
-            for (uint32_t g = 0; g < B.n; g++) {
-                const uint32_t m = m_first[b] + g;
-                for (uint32_t c = 0; c <= nc; c++) { off[(size_t)c * NM + m] = B.off[(size_t)c * B.n + g]; len[(size_t)c * NM + m] = B.len[(size_t)c * B.n + g]; }
-                rows[m] = B.rows[g]; reg[m] = 2 + (uint32_t)b; tmin[m] = B.tmin[g]; tmax[m] = B.tmax[g];
-            }
-        }
-        SegSrc &m = src[SRC_MERGED];
-        uint64_t *d_off; uint32_t *d_len, *d_rows, *d_reg; int64_t *d_tmin, *d_tmax;
-        if ((rc = m_own.get(&d_off, off.size())) || (rc = m_own.get(&d_len, len.size())) || (rc = m_own.get(&d_rows, NM)) || (rc = m_own.get(&d_reg, NM)) ||
-            (rc = m_own.get(&d_tmin, NM)) || (rc = m_own.get(&d_tmax, NM)))
-            return rc;
-        CU(cudaMemcpy(d_off, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(d_len, len.data(), len.size() * 4, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(d_rows, rows.data(), NM * 4ull, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(d_reg, reg.data(), NM * 4ull, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(d_tmin, tmin.data(), NM * 8ull, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(d_tmax, tmax.data(), NM * 8ull, cudaMemcpyHostToDevice));
-        m = SegSrc{d_off, d_len, d_rows, d_tmin, d_tmax, d_reg, 0, d_identity, NM, nc};
-    }
+    if ((rc = batches_source(batches, nc, d_identity, 2, regions, m_own, src[SRC_MERGED], m_first))) return rc;
     /* ---- the new directory as runs: per series the shard's segments before its span, new ordered ones before it, the span's
        merged segments, then the rest of both ---- */
     std::vector<Run> runs;
@@ -853,23 +885,7 @@ static int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *fi
     if (!sd.data) { sd.data = nw->d_data; sd.data_len = nw->data_len; nw->d_data = nullptr; out_own.bufs.push_back(sd.data); }
     CU(cudaEventRecord(ev1, 0));
     /* ---- derived state ---- */
-    {
-        Scratch t;
-        unsigned long long *d_tot; uint32_t *d_max; long long *d_range; int *d_err;
-        if ((rc = t.get(&d_tot, 3)) || (rc = t.get(&d_max, 1)) || (rc = t.get(&d_range, 2)) || (rc = t.get(&d_err, 2))) return rc;
-        const long long r0[2] = {INT64_MAX, INT64_MIN};
-        CU(cudaMemset(d_tot, 0, 24)); CU(cudaMemset(d_max, 0, 4)); CU(cudaMemset(d_err, 0, 8));
-        CU(cudaMemcpy(d_range, r0, 16, cudaMemcpyHostToDevice));
-        if (NOUT) k_append_stats<<<(NOUT + 127) / 128, 128>>>(sd.data, sd.off, sd.len, sd.rows, sd.tmin, sd.tmax, NOUT, nc, d_tot, d_max, d_range, d_err);
-        CU(cudaGetLastError());
-        unsigned long long tot[3]; long long range[2]; int err[2];
-        CU(cudaMemcpy(tot, d_tot, 24, cudaMemcpyDeviceToHost));
-        CU(cudaMemcpy(&out->max_seg_rows, d_max, 4, cudaMemcpyDeviceToHost));
-        CU(cudaMemcpy(range, d_range, 16, cudaMemcpyDeviceToHost));
-        CU(cudaMemcpy(err, d_err, 8, cudaMemcpyDeviceToHost));
-        if (err[0]) { set_error("segment %d: time page failed to parse after the append (device code %d)", err[1], err[0]); return OG_E_CORRUPT; }
-        out->n_rows = tot[0]; out->page_bytes = tot[1]; out->irregular_time_pages = tot[2]; out->tmin = range[0]; out->tmax = range[1];
-    }
+    if ((rc = spliced_totals(sd, nc, *out, "the append"))) return rc;
     /* the Snappy counters hold while every transcoded page is in the shard: the first merge drops them */
     out->rows_merged = s->rows_merged || !batches.empty();
     if (!out->rows_merged) {
@@ -887,10 +903,7 @@ static int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *fi
     CU(cudaEventElapsedTime(&ms, ev0, ev1));
     info.merge_ms = ms;
     info.rows_after_merge = out->n_rows;
-    auto take = [](Scratch &own, void *p) { own.bufs.erase(std::find(own.bufs.begin(), own.bufs.end(), p)); };
-    for (void *p : {(void *)sd.off, (void *)sd.len, (void *)sd.rows, (void *)sd.series, (void *)sd.tmin, (void *)sd.tmax, (void *)sd.data}) take(out_own, p);
-    out->d_page_off = sd.off; out->d_page_len = sd.len; out->d_seg_rows = sd.rows; out->d_seg_series = sd.series; out->d_tmin = sd.tmin; out->d_tmax = sd.tmax;
-    out->d_data = sd.data; out->data_len = sd.data_len; out->owns_data = true;
+    take_spliced(out_own, sd, *out);
     out->merge = info;
     CU(cudaDeviceSynchronize());
     /* swap the whole state: `out` takes the old one and frees it on return (the caller's buffer of a shard opened in place is not

@@ -135,6 +135,15 @@ class Shard:
         self._with_file_descs(files, call)
         return self
 
+    def compact(self, rows_per_segment=0):
+        """Re-cut every series into full segments of rows_per_segment rows (0: 1000), the last one 1..rows_per_segment, every
+        column of a series with a page in each (og_shard_compact).  Returns the og_compact_info counters as a dict; all zero when
+        the shard was already compact."""
+        d = L.CompactDesc(rows_per_segment, 0)
+        info = L.CompactInfo()
+        L.check(L.lib().og_shard_compact(self.h, C.byref(d), C.byref(info)), "og_shard_compact")
+        return {k: getattr(info, k) for k, _ in L.CompactInfo._fields_}
+
     def merge_info(self):
         m = L.MergeInfo()
         L.check(L.lib().og_shard_merge_info(self.h, C.byref(m)), "og_shard_merge_info")
