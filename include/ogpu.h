@@ -366,7 +366,10 @@ OG_API void og_query_destroy(og_query *q);
 
 /* merge another shard's dense partial (same query shape) into q's dense result on the device:
  * used after an all-gather for selector aggregates whose (value,time) tie-breaks are not a plain NCCL op
- * (lib/record/reccord_functions.go:482-494).  `other` holds device pointers laid out like og_query_dense's. */
+ * (lib/record/reccord_functions.go:482-494).  `other` holds device pointers laid out like og_query_dense's.
+ * OG_E_INVAL, leaving q's record unchanged, when `other` differs in its shape, its grid (create both queries with
+ * OG_Q_QUERY_GRID), which columns carry times, or in any column's func or type (as og_query_dense reports them: a count is
+ * OG_TYPE_INT whatever column it counts, so counts of columns of different types merge). */
 OG_API int og_query_merge_dense(og_query *q, const og_dense_view *other);
 
 /* ---- cross-shard merge over NCCL (one shard per GPU, one process per GPU) ----

@@ -1000,6 +1000,12 @@ OG_API int og_query_merge_dense(og_query *q, const og_dense_view *other) {
     GroupP mine, oth; memset(&mine, 0, sizeof mine); memset(&oth, 0, sizeof oth);
     mine.n_groups = oth.n_groups = q->n_groups;
     for (uint32_t c = 0; c < p.n_calls; c++) {
+        /* the cells are raw bits: a record of other calls or types would be read as this one's (a count as a sum, int bits as doubles) */
+        if (other->cols[c].func != p.calls[c].func || other->cols[c].type != p.calls[c].out_type) {
+            set_error("dense column %u: func %d type %d, this query's is func %d type %d", c, other->cols[c].func, other->cols[c].type, p.calls[c].func,
+                      p.calls[c].out_type);
+            return OG_E_INVAL;
+        }
         mine.dense[c] = q->dense[c];
         oth.dense[c].val = (uint64_t *)other->cols[c].values; oth.dense[c].ok = other->cols[c].valid; oth.dense[c].tim = other->cols[c].times;
         if ((q->dense[c].tim != nullptr) != (oth.dense[c].tim != nullptr)) { set_error("dense column %u: times presence differs", c); return OG_E_INVAL; }
