@@ -261,6 +261,9 @@ OG_API void og_tssp_free(og_tssp *t);
 /* ---- shard ---- */
 OG_API int og_shard_open(const og_shard_desc *desc, og_shard **out);
 OG_API void og_shard_close(og_shard *s); /* queries of a closed shard may still be destroyed (og_query_destroy), not run */
+/* page_bytes: the field and time pages as the files stored them (a Snappy page at its stored size, though it is held transcoded
+ * to a raw page) while every transcoded page is still in the shard, that is until the first append that merges rows or the first
+ * compaction that re-cuts a series; from then on, later appends included, the pages as the shard holds them. */
 OG_API int og_shard_info(const og_shard *s, uint64_t *n_series, uint64_t *n_segments, uint64_t *n_rows,
                          uint64_t *page_bytes, int64_t *tmin, int64_t *tmax);
 

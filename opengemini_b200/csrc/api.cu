@@ -109,7 +109,7 @@ int shard_finalize(og_shard *s, bool scan_snappy) {
         set_error("segment %d: %s page (device validation code %d)", err[1], err[0] == D_UNSUPPORTED ? "unsupported codec in" : err[0] == D_TYPE ? "type mismatch in" : "corrupt", err[0]);
         return map_dev_err(err[0]);
     }
-    s->n_rows = tot[0]; s->page_bytes = tot[1] - s->snappy_bytes_out + s->snappy_bytes_in; /* algorithmic bytes = the pages as stored */
+    s->n_rows = tot[0]; s->page_bytes = tot[1] - s->snappy_bytes_out + s->snappy_bytes_in; /* algorithmic bytes = the pages as the files stored them (ogpu.h og_shard_info) */
     s->max_seg_rows = mx; s->irregular_time_pages = tot[2];
     return OG_OK;
 }
@@ -932,10 +932,15 @@ OG_API int og_query_run(og_query *q) {
     stt.dir_bytes = (uint64_t)segs_scanned * 32; /* SURVEY §8d accounting: 32 B of directory per scanned segment */
     stt.out_bytes = 0;
     for (uint32_t c = 0; c < p.n_calls; c++) stt.out_bytes += cells_dense * (9 + (q->dense[c].tim ? 8 : 0));
-    if (p.n_cols == 1 && p.col_type[0] == OG_TYPE_FLOAT && p.col_index[0] < (int)s->il.size()) {
-        const og_shard::IlCol &ic = s->il[p.col_index[0]];
-        stt.il_state = ic.state; stt.il_build_ms = ic.build_ms; stt.il_bytes = ic.n_words * 4; stt.il_packed_segments = ic.state == 1 ? ic.n_packed : 0;
-        stt.general_segments = ic.state == 1 ? (uint64_t)ic.gen_host.size() : s->n_segments;
+    if (p.n_cols == 1 && p.col_type[0] == OG_TYPE_FLOAT) {
+        /* a query of another thread may be building this copy (ensure_il marks it -1 until it is ready): read it under the
+           build's lock, so a query never reports a half-built copy as "no eligible page" */
+        std::lock_guard<std::mutex> il_lock(s->il_mu);
+        if (p.col_index[0] < (int)s->il.size()) {
+            const og_shard::IlCol &ic = s->il[p.col_index[0]];
+            stt.il_state = ic.state; stt.il_build_ms = ic.build_ms; stt.il_bytes = ic.n_words * 4; stt.il_packed_segments = ic.state == 1 ? ic.n_packed : 0;
+            stt.general_segments = ic.state == 1 ? (uint64_t)ic.gen_host.size() : s->n_segments;
+        }
     }
     stt.per_series_cells_used = err[2] != 0;
     q->ran = true;
