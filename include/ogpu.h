@@ -321,6 +321,58 @@ OG_API int og_shard_merge_info(const og_shard *s, og_merge_info *out); /* og_sha
  *   (OG_SHARD_DEVICE_DATA) gets its own buffer; the caller's buffer is never written. */
 OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files);
 
+/* ---- rows into a shard: the flush of a memtable snapshot (csrc/flush.cu).  Replaces the device-side half of the reference's
+ * memtable flush (engine/mutable/ts_table.go:63-133 FlushChunks): sort each series' record, split it at the series' last flushed
+ * time, encode both parts into an ordered and an out-of-order file (MsBuilder.WriteRecord -> WriteData, engine/immutable/
+ * msbuilder.go:1151), and add the files to the shard.  Here the rows go to the device once and are sorted, split and encoded
+ * there; the files never exist on the host.
+ *   Sort and deduplicate per series (WriteChunk.SortRecord -> ColumnSortHelper.Sort, lib/record/column_sort.go:42-97): rows
+ *   sorted stably by time; for a run of equal times each column takes the last non-null value in arrival order, a null never
+ *   replaces a value (replace, :100-107).
+ *   Split (SplitRecordByTime, engine/mutable/ts_table.go:242-290): `last` is the latest time the shard holds for the series,
+ *   INT64_MIN for a sid it lacks (MmsIdTime.get, engine/immutable/sequencer.go:92-101); rows with t > last form the ordered part,
+ *   rows with t <= last the out-of-order part.  A column with no non-null value in a part is left out of that part (no page for
+ *   the series in that file, ts_table.go:276-286), not written as an all-null page.
+ *   Cut each part into 1000-row segments from its first row (WriteData; lib/util/util.go:72); every column kept in the part has
+ *   a page in every segment, from the encoders of og_encode_pages (raw page for a float segment Gorilla refuses).
+ *   Join the shard: afterwards the shard answers every entry point, byte for byte, as og_shard_append_files of those two files
+ *   (ordered first, each only when it holds rows) would, og_shard_merge_info included (apart from merge_ms): the call reports
+ *   as an append of its non-empty files.
+ * Refused, the shard left as it was (only its interleaved copies may have been dropped; rebuilt on first use): a string field
+ * (OG_E_UNSUPPORTED, naming it: there is no device string encoder); a field whose type differs from the shard's column of that
+ * name (OG_E_TYPE); no rows, sid 0, a repeated sid or field name, a column whose len is neither 0 nor rows, a nil_count that
+ * disagrees with the bitmap, val_bytes that disagree with len - nil_count, or non-zero flags (OG_E_INVAL); a live og_query of
+ * the shard (OG_E_STATE; og_query_create on another thread waits while the flush runs).
+ * Cost: one host-to-device copy per batch of series (batches under the merge's device-memory budget, each series charged its rows
+ * and the 1000-row segment slots of its parts; OGPU_MERGE_BATCH_ROWS overrides the budget); the
+ * out-of-order part is encoded here and decoded once more by the merge of og_shard_append_files. ---- */
+typedef struct og_rows_field { const char *name; int32_t type; } og_rows_field; /* OG_TYPE_INT / FLOAT / BOOL */
+typedef struct og_rows_series {
+    uint64_t sid;               /* non-zero, unique in the call */
+    uint32_t rows;
+    const int64_t *times;       /* [rows] in arrival order: unsorted, equal times allowed */
+    const og_colval_view *cols; /* [n_fields] in field order, the ColVal layout: val = non-null values packed densely (8 bytes
+                                   each, 1 for bool), bitmap LSB-first from bitmap_offset (NULL allowed when nil_count == 0),
+                                   len == rows, nil_count, type == the field's type, times NULL.  len == 0: the series has no
+                                   such column in this call (all its rows null) */
+} og_rows_series;
+typedef struct og_rows_desc {
+    uint32_t n_fields; const og_rows_field *fields; /* names unique */
+    uint32_t n_series; const og_rows_series *series;
+    uint32_t flags;                                 /* 0 */
+} og_rows_desc;
+typedef struct og_rows_info {
+    uint64_t series_in, rows_in;
+    uint64_t rows_replaced;     /* rows a later row of the same series and time replaced (deduplication inside the call) */
+    uint64_t ordered_rows, out_of_order_rows;
+    uint64_t segments_written;  /* segments of the two flushed files */
+    double phase_ms[4];         /* wall clock: [0] rows staged and copied to the device, [1] expand + sort + split + runs of equal
+                                   times, [2] combine + encode + the pages gathered into the two files, [3] add_files */
+} og_rows_info;
+OG_API int og_shard_append_rows(og_shard *s, const og_rows_desc *rows, og_rows_info *info /* may be NULL */);
+/* a flush into an empty shard, as og_shard_open_files is an append to one */
+OG_API int og_shard_open_rows(const og_rows_desc *rows, og_shard **out, og_rows_info *info /* may be NULL */);
+
 /* ---- compaction of an open shard (csrc/compact.cu).  Replaces the device pass of the reference's non-streaming level
  * compaction (engine/immutable/compact.go:175-242): a series' merged records written through MsBuilder.WriteRecord -> WriteData
  * (msbuilder.go:1151), which cuts them into segments of R rows from the start of the series, every column of the chunk schema

@@ -121,6 +121,24 @@ class CompactInfo(C.Structure):
                 ("segments_rewritten_out", C.c_uint64), ("rows_rewritten", C.c_uint64), ("compact_ms", C.c_double)]
 
 
+class RowsField(C.Structure):
+    _fields_ = [("name", C.c_char_p), ("type", C.c_int32)]
+
+
+class RowsSeries(C.Structure):
+    _fields_ = [("sid", C.c_uint64), ("rows", C.c_uint32), ("times", i64p), ("cols", C.POINTER(ColValView))]
+
+
+class RowsDesc(C.Structure):
+    _fields_ = [("n_fields", C.c_uint32), ("fields", C.POINTER(RowsField)), ("n_series", C.c_uint32),
+                ("series", C.POINTER(RowsSeries)), ("flags", C.c_uint32)]
+
+
+class RowsInfo(C.Structure):
+    _fields_ = [("series_in", C.c_uint64), ("rows_in", C.c_uint64), ("rows_replaced", C.c_uint64), ("ordered_rows", C.c_uint64),
+                ("out_of_order_rows", C.c_uint64), ("segments_written", C.c_uint64), ("phase_ms", C.c_double * 4)]
+
+
 class TsspWriteDesc(C.Structure):
     _fields_ = [("measurement", C.c_char_p), ("series_begin", C.c_uint32), ("series_end", C.c_uint32), ("flags", C.c_uint32)]
 
@@ -136,6 +154,7 @@ EXPORTS = [
     "og_downsample_shard", "og_downsampled_timing",
     "og_tssp_parse", "og_tssp_desc", "og_tssp_measurement", "og_tssp_time_range", "og_tssp_free",
     "og_shard_open_files", "og_shard_merge_info", "og_shard_append_files", "og_shard_compact",
+    "og_shard_append_rows", "og_shard_open_rows",
     "og_shard_write_tssp", "og_tssp_image_size", "og_tssp_image_export", "og_tssp_image_timing", "og_tssp_image_free",
 ]
 
@@ -167,6 +186,8 @@ def lib():
     L.og_shard_open_files.argtypes = [C.POINTER(ShardDesc), u32p, C.c_uint32, C.POINTER(C.c_void_p)]
     L.og_shard_merge_info.argtypes = [C.c_void_p, C.POINTER(MergeInfo)]
     L.og_shard_append_files.argtypes = [C.c_void_p, C.POINTER(ShardDesc), u32p, C.c_uint32]
+    L.og_shard_append_rows.argtypes = [C.c_void_p, C.POINTER(RowsDesc), C.POINTER(RowsInfo)]
+    L.og_shard_open_rows.argtypes = [C.POINTER(RowsDesc), C.POINTER(C.c_void_p), C.POINTER(RowsInfo)]
     L.og_shard_compact.argtypes = [C.c_void_p, C.POINTER(CompactDesc), C.POINTER(CompactInfo)]
     L.og_shard_close.argtypes = [C.c_void_p]
     L.og_shard_close.restype = None

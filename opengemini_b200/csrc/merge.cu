@@ -1,7 +1,9 @@
 /*
  * merge.cu — TSSP files into a shard (DESIGN.md (d) "Bringing files into a shard").  og_shard_open_files opens the ordered and
  * out-of-order files of one shard as ONE og_shard; og_shard_append_files adds files flushed into an open shard.  An open is an
- * append to an empty shard: both run add_files.
+ * append to an empty shard: both run add_files.  add_files takes new files from one of two producers: upload_files (host files
+ * copied in, validated, transcoded) or place_files (the files og_shard_append_rows encoded on the device, flush.cu); everything
+ * from the probe on is one path for both.
  *
  * The reference merges a shard's files for every series of every query (include/ogpu.h lists the code).  Here the merge runs
  * once, when the files join the shard:
@@ -59,7 +61,6 @@ int encode_pages(int32_t type, int32_t is_time, const void *d_values, const uint
                  uint32_t rps, uint8_t *d_out, uint64_t out_cap, uint64_t *d_page_off, uint32_t *d_page_len, uint64_t *total_bytes_out,
                  bool nan_raw); /* encode.cu */
 
-#define MERGE_RPS 1000u           /* rows per rewritten segment: lib/util/util.go:72 */
 
 __device__ __forceinline__ bool merge_claim(MergeErr *e, int code) { return atomicCAS(&e->code, 0, code) == 0; }
 
@@ -124,12 +125,13 @@ __global__ void k_merge_span_out(const uint32_t *span_row0, uint32_t n_spans, co
     if (s <= n_spans) out_begin[s] = oidx[span_row0[s]];
 }
 
-/* one thread per run of equal times: the row rule, then the merged row into its 1000-row segment slot */
+/* one thread per run of equal times: the row rule, then the merged row into its 1000-row segment slot.  span_has (may be null):
+ * [span][column] set where the column holds a value in the span */
 __global__ void k_merge_combine(const int64_t *t, const uint32_t *perm, const uint32_t *row_span, const uint32_t *head,
                                 const uint32_t *oidx, const uint32_t *out_begin, const uint32_t *seg_base, const int32_t *col_types,
                                 uint32_t n_cols, uint32_t R, const uint64_t *cells, const uint8_t *ok, int64_t *out_t,
                                 uint8_t *const *out_cells, uint8_t *out_ok, size_t out_rows, int64_t *seg_tmin, int64_t *seg_tmax,
-                                unsigned long long *replaced) {
+                                unsigned long long *replaced, uint8_t *span_has) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= R || !head[i]) return;
     const uint32_t s = row_span[i], local = oidx[i] - out_begin[s], cnt = out_begin[s + 1] - out_begin[s];
@@ -147,6 +149,7 @@ __global__ void k_merge_combine(const int64_t *t, const uint32_t *perm, const ui
             if (ok[src]) { v = cells[src]; has = 1; }
         }
         out_ok[(size_t)c * out_rows + dst] = has;
+        if (has && span_has) span_has[(size_t)s * n_cols + c] = 1;
         if (col_types[c] == OG_TYPE_BOOL) out_cells[c][dst] = (uint8_t)v;
         else ((uint64_t *)out_cells[c])[dst] = v;
     }
@@ -163,6 +166,74 @@ struct Span {
     uint32_t batch = 0, first_new = 0, n_new = 0; /* new segments [first_new, first_new + n_new) of batch `batch` */
 };
 
+/* ---------------------------------------------------------------- sort, runs and the row rule (shared with the flush) */
+
+int sort_spans(const int64_t *times, int64_t *times_sorted, uint32_t *perm_in, uint32_t *perm, uint32_t R, uint32_t n_spans,
+               const uint32_t *d_span_row0, Scratch &b) {
+    int rc;
+    k_merge_iota<<<(R + 255) / 256, 256>>>(perm_in, R);
+    size_t tb = 0; void *tmp = nullptr;
+    CU(cub::DeviceSegmentedSort::StableSortPairs(nullptr, tb, times, times_sorted, perm_in, perm, (int)R, (int)n_spans, d_span_row0, d_span_row0 + 1));
+    if ((rc = b.get((uint8_t **)&tmp, tb))) return rc;
+    CU(cub::DeviceSegmentedSort::StableSortPairs(tmp, tb, times, times_sorted, perm_in, perm, (int)R, (int)n_spans, d_span_row0, d_span_row0 + 1));
+    return OG_OK;
+}
+
+int find_runs(SortedRows &r, const uint32_t *row_file, Scratch &b, MergeErr *d_err) {
+    int rc;
+    if ((rc = b.get(&r.head, (size_t)r.R + 1)) || (rc = b.get(&r.oidx, (size_t)r.R + 1)) || (rc = b.get(&r.out_begin, r.n_spans + 1))) return rc;
+    k_merge_heads<<<(r.R + 1 + 255) / 256, 256>>>(r.t, r.perm, row_file, r.row_span, r.R, r.head, d_err);
+    {
+        size_t tb = 0; void *tmp = nullptr;
+        CU(cub::DeviceScan::ExclusiveSum(nullptr, tb, r.head, r.oidx, (int)r.R + 1));
+        if ((rc = b.get((uint8_t **)&tmp, tb))) return rc;
+        CU(cub::DeviceScan::ExclusiveSum(tmp, tb, r.head, r.oidx, (int)r.R + 1));
+    }
+    k_merge_span_out<<<(r.n_spans + 1 + 127) / 128, 128>>>(r.span_row0, r.n_spans, r.oidx, r.out_begin);
+    CU(cudaGetLastError());
+    return OG_OK;
+}
+
+int combine_and_encode(const SortedRows &r, const std::vector<int32_t> &types, const int32_t *d_types, Scratch &b, unsigned long long *d_rep,
+                       uint8_t *span_has, Scratch &blobs, NewSegs &ns, std::vector<uint32_t> &seg_first) {
+    int rc;
+    const uint32_t nc = (uint32_t)types.size(), ncol1 = nc + 1, nsp = r.n_spans;
+    std::vector<uint32_t> h_out(nsp + 1), h_rows;
+    CU(cudaMemcpy(h_out.data(), r.out_begin, (nsp + 1) * 4ull, cudaMemcpyDeviceToHost));
+    seg_first.assign(nsp + 1, 0);
+    for (uint32_t k = 0; k < nsp; k++) {
+        const uint32_t cnt = h_out[k + 1] - h_out[k], nseg = (cnt + MERGE_RPS - 1) / MERGE_RPS;
+        seg_first[k + 1] = seg_first[k] + nseg;
+        for (uint32_t g = 0; g < nseg; g++) h_rows.push_back(std::min(MERGE_RPS, cnt - g * MERGE_RPS));
+    }
+    const uint32_t NS = ns.n = seg_first[nsp];
+    const size_t out_rows = (size_t)NS * MERGE_RPS;
+    int64_t *out_t, *d_tmin, *d_tmax; uint8_t *out_ok; uint32_t *d_rows, *seg_base; uint8_t **d_cols;
+    std::vector<uint8_t *> h_cols(nc);
+    if ((rc = b.get(&out_t, out_rows)) || (rc = b.get(&out_ok, (size_t)nc * out_rows)) || (rc = b.get(&d_tmin, NS)) ||
+        (rc = b.get(&d_tmax, NS)) || (rc = b.get(&d_rows, NS)) || (rc = b.get(&d_cols, nc)) || (rc = b.get(&seg_base, nsp)))
+        return rc;
+    for (uint32_t c = 0; c < nc; c++)
+        if ((rc = b.get(&h_cols[c], out_rows * (types[c] == OG_TYPE_BOOL ? 1 : 8)))) return rc;
+    CU(cudaMemcpy(d_cols, h_cols.data(), nc * sizeof(uint8_t *), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(seg_base, seg_first.data(), nsp * 4ull, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_rows, h_rows.data(), NS * 4ull, cudaMemcpyHostToDevice));
+    k_merge_combine<<<(r.R + 127) / 128, 128>>>(r.t, r.perm, r.row_span, r.head, r.oidx, r.out_begin, seg_base, d_types, nc, r.R, r.cells, r.ok,
+                                                 out_t, d_cols, out_ok, out_rows, d_tmin, d_tmax, d_rep, span_has);
+    CU(cudaGetLastError());
+    /* encode every column (string columns: no values inside a span, so no page) */
+    uint8_t *blob;
+    const uint64_t cap = (uint64_t)NS * ncol1 * MERGE_PAGE_BOUND;
+    if ((rc = b.get(&blob, cap))) return rc;
+    uint64_t used = 0;
+    if ((rc = encode_columns(types, out_t, h_cols, out_ok, out_rows, d_rows, NS, MERGE_RPS, blob, cap, ns, &used))) return rc;
+    ns.tmin.resize(NS); ns.tmax.resize(NS); ns.rows = h_rows;
+    CU(cudaMemcpy(ns.tmin.data(), d_tmin, NS * 8ull, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(ns.tmax.data(), d_tmax, NS * 8ull, cudaMemcpyDeviceToHost));
+    /* keep only the bytes written: the batch's scratch goes back to the pool before the next batch */
+    return keep_blob(blob, used, blobs, ns);
+}
+
 /* Merge every span on the device, batch by batch: the spans' source segments are read through `dir`, whose columns are `types` /
  * `names` and whose segments `dir_runs` spliced from the shard and the files.  Fills batches[] and each span's new-segment range.
  * A repeated time names its file, or the shard's rows when the file is `shard_file`.  Every batch's blob is followed by 1024
@@ -170,14 +241,10 @@ struct Span {
 static int merge_spans(const SrcDir &dir, const std::vector<Run> &dir_runs, const std::vector<int32_t> &types, const std::vector<std::string> &names,
                        const std::vector<Span *> &spans, const std::vector<uint64_t> &sids, uint32_t shard_file, std::vector<NewSegs> &batches,
                        Scratch &blobs, uint64_t *replaced_out) {
-    const uint32_t nc = dir.n_columns, ncol1 = nc + 1;
+    const uint32_t nc = dir.n_columns;
     int rc;
-    /* scratch per row: decode (8 t + 4 file + 4 span + 9 per column), sort (4 + 4 perm, 8 keys), heads + scan (8), output slots
-       (8 + 9 per column), encoder staging and blob (2 x 8704 / 1000 per page) */
-    const uint64_t per_row = 48 + 18ull * nc + 2ull * ncol1 * MERGE_PAGE_BOUND / MERGE_RPS + 64;
     uint64_t cap_rows;
-    if ((rc = batch_cap_rows(per_row, MERGE_RPS, "OGPU_MERGE_BATCH_ROWS", &cap_rows))) return rc;
-    std::vector<int64_t> h_zero;
+    if ((rc = batch_cap_rows(span_row_bytes(nc), MERGE_RPS, "OGPU_MERGE_BATCH_ROWS", &cap_rows))) return rc;
     unsigned long long *d_rep; MergeErr *d_err; int32_t *d_types;
     Scratch keep;
     if ((rc = keep.get(&d_rep, 1)) || (rc = keep.get(&d_err, 1)) || (rc = keep.get(&d_types, nc))) return rc;
@@ -200,14 +267,12 @@ static int merge_spans(const SrcDir &dir, const std::vector<Run> &dir_runs, cons
         h_span_row0.push_back(row);
         const uint32_t nsrc = (uint32_t)h_seg.size();
         Scratch b;
-        uint32_t *d_seg, *d_row0, *d_file, *d_span, *d_span_row0, *row_file, *row_span, *perm_in, *perm, *head, *oidx, *out_begin, *seg_base;
+        uint32_t *d_seg, *d_row0, *d_file, *d_span, *d_span_row0, *row_file, *row_span, *perm_in, *perm;
         int64_t *times, *times_sorted; uint64_t *cells; uint8_t *ok;
         if ((rc = b.get(&d_seg, nsrc)) || (rc = b.get(&d_row0, nsrc)) || (rc = b.get(&d_file, nsrc)) || (rc = b.get(&d_span, nsrc)) ||
             (rc = b.get(&d_span_row0, nsp + 1)) || (rc = b.get(&row_file, R)) || (rc = b.get(&row_span, R)) ||
-            (rc = b.get(&perm_in, R)) || (rc = b.get(&perm, R)) || (rc = b.get(&head, (size_t)R + 1)) ||
-            (rc = b.get(&oidx, (size_t)R + 1)) || (rc = b.get(&out_begin, nsp + 1)) || (rc = b.get(&seg_base, nsp)) ||
-            (rc = b.get(&times, R)) || (rc = b.get(&times_sorted, R)) || (rc = b.get(&cells, (size_t)nc * R)) ||
-            (rc = b.get(&ok, (size_t)nc * R)))
+            (rc = b.get(&perm_in, R)) || (rc = b.get(&perm, R)) || (rc = b.get(&times, R)) || (rc = b.get(&times_sorted, R)) ||
+            (rc = b.get(&cells, (size_t)nc * R)) || (rc = b.get(&ok, (size_t)nc * R)))
             return rc;
         CU(cudaMemcpy(d_seg, h_seg.data(), nsrc * 4ull, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(d_row0, h_row0.data(), nsrc * 4ull, cudaMemcpyHostToDevice));
@@ -215,23 +280,11 @@ static int merge_spans(const SrcDir &dir, const std::vector<Run> &dir_runs, cons
         CU(cudaMemcpy(d_span, h_span.data(), nsrc * 4ull, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(d_span_row0, h_span_row0.data(), (nsp + 1) * 4ull, cudaMemcpyHostToDevice));
         k_merge_decode<<<(nsrc + 127) / 128, 128>>>(dir, d_types, nsrc, d_seg, d_row0, d_file, d_span, R, times, row_file, row_span, cells, ok, d_err);
-        k_merge_iota<<<(R + 255) / 256, 256>>>(perm_in, R);
-        { /* rows of a span by time; stable, so equal times keep file order */
-            size_t tb = 0; void *tmp = nullptr;
-            CU(cub::DeviceSegmentedSort::StableSortPairs(nullptr, tb, times, times_sorted, perm_in, perm, (int)R, (int)nsp, d_span_row0, d_span_row0 + 1));
-            if ((rc = b.get((uint8_t **)&tmp, tb))) return rc;
-            CU(cub::DeviceSegmentedSort::StableSortPairs(tmp, tb, times, times_sorted, perm_in, perm, (int)R, (int)nsp, d_span_row0, d_span_row0 + 1));
-        }
+        /* rows of a span by time; stable, so equal times keep file order */
+        if ((rc = sort_spans(times, times_sorted, perm_in, perm, R, nsp, d_span_row0, b))) return rc;
         /* row_span is constant over a span's rows, so it indexes sorted positions as well as decoded ones */
-        k_merge_heads<<<(R + 1 + 255) / 256, 256>>>(times_sorted, perm, row_file, row_span, R, head, d_err);
-        {
-            size_t tb = 0; void *tmp = nullptr;
-            CU(cub::DeviceScan::ExclusiveSum(nullptr, tb, head, oidx, (int)R + 1));
-            if ((rc = b.get((uint8_t **)&tmp, tb))) return rc;
-            CU(cub::DeviceScan::ExclusiveSum(tmp, tb, head, oidx, (int)R + 1));
-        }
-        k_merge_span_out<<<(nsp + 1 + 127) / 128, 128>>>(d_span_row0, nsp, oidx, out_begin);
-        CU(cudaGetLastError());
+        SortedRows sr{times_sorted, perm, row_span, d_span_row0, cells, ok, R, nsp};
+        if ((rc = find_runs(sr, row_file, b, d_err))) return rc;
         MergeErr he;
         CU(cudaMemcpy(&he, d_err, sizeof he, cudaMemcpyDeviceToHost));
         if (he.code) {
@@ -242,44 +295,13 @@ static int merge_spans(const SrcDir &dir, const std::vector<Run> &dir_runs, cons
             const Run &r = *std::prev(std::upper_bound(dir_runs.begin(), dir_runs.end(), (uint32_t)he.seg, [](uint32_t g, const Run &x) { return g < x.out0; }));
             return decode_failure(he.code, r.src0 + ((uint32_t)he.seg - r.out0), r.kind == SRC_SHARD ? "shard" : "file set");
         }
-        std::vector<uint32_t> h_out(nsp + 1), h_base(nsp);
-        CU(cudaMemcpy(h_out.data(), out_begin, (nsp + 1) * 4ull, cudaMemcpyDeviceToHost));
         NewSegs ns;
-        std::vector<uint32_t> h_rows;
+        std::vector<uint32_t> seg_first;
+        if ((rc = combine_and_encode(sr, types, d_types, b, d_rep, nullptr, blobs, ns, seg_first))) return rc;
         for (uint32_t k = 0; k < nsp; k++) {
-            const uint32_t cnt = h_out[k + 1] - h_out[k], nseg = (cnt + MERGE_RPS - 1) / MERGE_RPS;
             Span &sp = *spans[sp0 + k];
-            sp.batch = (uint32_t)batches.size(); sp.first_new = ns.n; sp.n_new = nseg;
-            h_base[k] = ns.n;
-            for (uint32_t g = 0; g < nseg; g++) h_rows.push_back(std::min(MERGE_RPS, cnt - g * MERGE_RPS));
-            ns.n += nseg;
+            sp.batch = (uint32_t)batches.size(); sp.first_new = seg_first[k]; sp.n_new = seg_first[k + 1] - seg_first[k];
         }
-        const uint32_t NS = ns.n;
-        const size_t out_rows = (size_t)NS * MERGE_RPS;
-        int64_t *out_t, *d_tmin, *d_tmax; uint8_t *out_ok; uint32_t *d_rows; uint8_t **d_cols;
-        std::vector<uint8_t *> h_cols(nc);
-        if ((rc = b.get(&out_t, out_rows)) || (rc = b.get(&out_ok, (size_t)nc * out_rows)) || (rc = b.get(&d_tmin, NS)) ||
-            (rc = b.get(&d_tmax, NS)) || (rc = b.get(&d_rows, NS)) || (rc = b.get(&d_cols, nc)))
-            return rc;
-        for (uint32_t c = 0; c < nc; c++)
-            if ((rc = b.get(&h_cols[c], out_rows * (types[c] == OG_TYPE_BOOL ? 1 : 8)))) return rc;
-        CU(cudaMemcpy(d_cols, h_cols.data(), nc * sizeof(uint8_t *), cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(seg_base, h_base.data(), nsp * 4ull, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(d_rows, h_rows.data(), NS * 4ull, cudaMemcpyHostToDevice));
-        k_merge_combine<<<(R + 127) / 128, 128>>>(times_sorted, perm, row_span, head, oidx, out_begin, seg_base, d_types, nc, R, cells, ok,
-                                                   out_t, d_cols, out_ok, out_rows, d_tmin, d_tmax, d_rep);
-        CU(cudaGetLastError());
-        /* encode every column (string columns: no values inside a span, so no page) */
-        uint8_t *blob;
-        const uint64_t cap = (uint64_t)NS * ncol1 * MERGE_PAGE_BOUND;
-        if ((rc = b.get(&blob, cap))) return rc;
-        uint64_t used = 0;
-        if ((rc = encode_columns(types, out_t, h_cols, out_ok, out_rows, d_rows, NS, MERGE_RPS, blob, cap, ns, &used))) return rc;
-        ns.tmin.resize(NS); ns.tmax.resize(NS); ns.rows = h_rows;
-        CU(cudaMemcpy(ns.tmin.data(), d_tmin, NS * 8ull, cudaMemcpyDeviceToHost));
-        CU(cudaMemcpy(ns.tmax.data(), d_tmax, NS * 8ull, cudaMemcpyDeviceToHost));
-        /* keep only the bytes written: the batch's scratch goes back to the pool before the next batch */
-        if ((rc = keep_blob(blob, used, blobs, ns))) return rc;
         batches.push_back(std::move(ns));
         sp0 = sp1;
     }
@@ -360,26 +382,50 @@ static int build_file_dir(const og_shard_desc *files, uint32_t n_files, const st
     return OG_OK;
 }
 
-/* the files' bytes in one device buffer (one H2D per file) under the directory of build_file_dir, validated and with their Snappy
- * pages transcoded (shard_finalize); fd.off / fd.len are updated to the transcoded directory, rows[] gets every segment's rows */
-static int upload_files(const og_shard_desc *files, uint32_t n_files, const std::vector<std::string> &names, const std::vector<int32_t> &types,
-                        int dev, FileDir &fd, std::unique_ptr<og_shard> &out, std::vector<uint32_t> &rows) {
-    int rc;
-    std::unique_ptr<og_shard> src(new og_shard);
+/* the new files' shard: the directory of build_file_dir over the union columns, on the device */
+static int new_files_shard(const og_shard_desc *files, uint32_t n_files, const std::vector<std::string> &names, const std::vector<int32_t> &types,
+                           int dev, const FileDir &fd, std::unique_ptr<og_shard> &out) {
+    out.reset(new og_shard);
+    og_shard *src = out.get();
     src->device = dev; src->n_series = (uint32_t)fd.ser0[n_files]; src->n_segments = fd.n; src->n_columns = (uint32_t)names.size();
     src->col_types = types; src->col_names = names; src->data_len = fd.data_len;
     src->h_series_seg_begin = fd.ssb;
     for (uint32_t f = 0; f < n_files; f++) src->sids.insert(src->sids.end(), files[f].sids, files[f].sids + files[f].n_series);
+    return upload_dir(src, fd.ssb.data(), fd.tmin.data(), fd.tmax.data(), fd.off.data(), fd.len.data(), src->sids.data());
+}
+
+/* one producer of new files on the device: the files' bytes in one device buffer (one H2D per file) under the directory of
+ * build_file_dir, validated and with their Snappy pages transcoded (shard_finalize); fd.off / fd.len are updated to the transcoded
+ * directory, rows[] gets every segment's rows */
+static int upload_files(const og_shard_desc *files, uint32_t n_files, const std::vector<std::string> &names, const std::vector<int32_t> &types,
+                        int dev, FileDir &fd, std::unique_ptr<og_shard> &out, std::vector<uint32_t> &rows) {
+    int rc;
+    std::unique_ptr<og_shard> src;
+    if ((rc = new_files_shard(files, n_files, names, types, dev, fd, src))) return rc;
     if ((rc = dalloc(&src->d_data, fd.data_len + 1024))) return rc;
     CU(cudaMemset(src->d_data, 0, fd.data_len + 1024));
     for (uint32_t f = 0; f < n_files; f++)
         if (files[f].data_len) CU(cudaMemcpy(src->d_data + fd.base[f], files[f].data, files[f].data_len, cudaMemcpyHostToDevice));
-    if ((rc = upload_dir(src.get(), fd.ssb.data(), fd.tmin.data(), fd.tmax.data(), fd.off.data(), fd.len.data(), src->sids.data()))) return rc;
     if ((rc = shard_finalize(src.get(), true))) return rc;
     CU(cudaMemcpy(fd.off.data(), src->d_page_off, fd.off.size() * 8, cudaMemcpyDeviceToHost));
     CU(cudaMemcpy(fd.len.data(), src->d_page_len, fd.len.size() * 4, cudaMemcpyDeviceToHost));
     rows.resize(fd.n);
     CU(cudaMemcpy(rows.data(), src->d_seg_rows, fd.n * 4ull, cudaMemcpyDeviceToHost));
+    out = std::move(src);
+    return OG_OK;
+}
+
+/* the other producer: files the flush encoded on the device (DeviceFiles), taken over as they lie */
+static int place_files(const og_shard_desc *files, uint32_t n_files, const std::vector<std::string> &names, const std::vector<int32_t> &types,
+                       int dev, const FileDir &fd, DeviceFiles &df, std::unique_ptr<og_shard> &out, std::vector<uint32_t> &rows) {
+    int rc;
+    if (df.data_len < fd.data_len || df.rows.size() != fd.n) { set_error("internal: the device files do not match their directory"); return OG_E_INVAL; }
+    std::unique_ptr<og_shard> src;
+    if ((rc = new_files_shard(files, n_files, names, types, dev, fd, src))) return rc;
+    if ((rc = dalloc(&src->d_seg_rows, fd.n))) return rc;
+    CU(cudaMemcpy(src->d_seg_rows, df.rows.data(), fd.n * 4ull, cudaMemcpyHostToDevice));
+    src->d_data = df.data; df.data = nullptr;
+    rows = df.rows;
     out = std::move(src);
     return OG_OK;
 }
@@ -495,6 +541,28 @@ __global__ void __launch_bounds__(APPEND_GATHER_THREADS) k_append_gather(const u
         *(uint4 *)(dst + head + 16 * k) = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
     }
     for (uint32_t i = tail + lane; i < l; i += 32) dst[i] = __ldg(src + i);
+}
+
+/* pages from regions[page_region[p]] + src_off[p] to out + dst_off[p] (len[p] bytes each) with k_append_gather: the flush's
+ * pages into the region of its files (flush.cu) */
+int gather_pages(const std::vector<const uint8_t *> &regions, const std::vector<uint32_t> &page_region, const std::vector<uint64_t> &src_off,
+                 const std::vector<uint32_t> &len, const std::vector<uint64_t> &dst_off, uint8_t *out) {
+    int rc;
+    const uint64_t n = len.size();
+    if (!n) return OG_OK;
+    Scratch t;
+    const uint8_t **d_regions; uint32_t *d_reg, *d_len; uint64_t *d_src, *d_dst;
+    if ((rc = t.get(&d_regions, regions.size())) || (rc = t.get(&d_reg, n)) || (rc = t.get(&d_len, n)) || (rc = t.get(&d_src, n)) || (rc = t.get(&d_dst, n))) return rc;
+    CU(cudaMemcpy(d_regions, regions.data(), regions.size() * sizeof(void *), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_reg, page_region.data(), n * 4, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_len, len.data(), n * 4, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_src, src_off.data(), n * 8, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_dst, dst_off.data(), n * 8, cudaMemcpyHostToDevice));
+    k_append_gather<<<(unsigned)((n * 32 + APPEND_GATHER_THREADS - 1) / APPEND_GATHER_THREADS), APPEND_GATHER_THREADS>>>(
+        d_regions, d_reg, d_src, d_len, d_dst, (uint32_t)n, n, out);
+    CU(cudaGetLastError());
+    CU(cudaDeviceSynchronize()); /* t goes back to the pool */
+    return OG_OK;
 }
 
 /* per probed series of the shard: its last time, and the range [a, b) of its segments that a span [lo, hi] overlaps */
@@ -694,8 +762,8 @@ void take_spliced(Scratch &own, Spliced &sd, ShardState &out) {
 
 /* ---------------------------------------------------------------- files into a shard */
 
-/* the files join `s`: og_shard_append_files, and og_shard_open_files on an empty shard.  `who` names the caller in refusals. */
-static int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, const char *who) {
+/* the files join `s` (span_pass.h).  Everything from the probe on is one path for both producers of the new files. */
+int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, const char *who, DeviceFiles *dev) {
     int rc;
     /* ---- checks; schema union with the shard's columns (sorted by name), series union with its sids (ascending) ---- */
     const uint32_t onc = s->n_columns, ONSER = s->n_series, ONSEG = s->n_segments;
@@ -782,10 +850,12 @@ static int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *fi
         span_of[u] = (int)span_store.size();
         span_store.push_back(std::move(sp));
     }
-    /* ---- upload, validate and transcode the new files only ---- */
+    /* ---- the new files on the device: uploaded, validated and transcoded, or taken over from the flush ---- */
     std::unique_ptr<og_shard> nw;
     std::vector<uint32_t> new_rows;
-    if ((rc = upload_files(files, n_files, names, types, s->device, fd, nw, new_rows))) return rc;
+    if ((rc = dev ? place_files(files, n_files, names, types, s->device, fd, *dev, nw, new_rows)
+                  : upload_files(files, n_files, names, types, s->device, fd, nw, new_rows)))
+        return rc;
     /* the interleaved copies describe the old layout: dropped now, rebuilt by the first query that wants them */
     {
         std::lock_guard<std::mutex> il_lock(s->il_mu);
@@ -929,7 +999,7 @@ OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_
     std::unique_ptr<og_shard> s(new og_shard); /* an open is an append to an empty shard */
     CU(cudaGetDevice(&s->device));
     s->h_series_seg_begin = {0};
-    if ((rc = add_files(s.get(), files, file_flags, n_files, "og_shard_open_files"))) return rc;
+    if ((rc = add_files(s.get(), files, file_flags, n_files, "og_shard_open_files", nullptr))) return rc;
     *out = s.release();
     return OG_OK;
 }
@@ -939,7 +1009,7 @@ OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const 
     std::lock_guard<std::mutex> lock(s->live->mu); /* og_query_create waits until the append is done */
     if (s->live->n) { set_error("%u queries on this shard are still open: destroy them before appending files", s->live->n); return OG_E_STATE; }
     CU(cudaSetDevice(s->device));
-    return add_files(s, files, file_flags, n_files, "og_shard_append_files");
+    return add_files(s, files, file_flags, n_files, "og_shard_append_files", nullptr);
 }
 
 OG_API int og_shard_merge_info(const og_shard *s, og_merge_info *out) {

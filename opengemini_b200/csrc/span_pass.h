@@ -63,6 +63,52 @@ int encode_columns(const std::vector<int32_t> &types, const int64_t *d_times, co
  * past a page's end) */
 int keep_blob(const uint8_t *blob, uint64_t used, Scratch &blobs, NewSegs &ns);
 
+#define MERGE_RPS 1000u /* rows per rewritten segment: lib/util/util.go:72 */
+
+/* device scratch per row of a batch of nc columns: decode (8 t + 4 file + 4 span + 9 per column), sort (4 + 4 perm, 8 keys), heads +
+   scan (8), output slots (8 + 9 per column), encoder staging and blob (2 x 8704 / 1000 per page) */
+inline uint64_t span_row_bytes(uint32_t nc) { return 48 + 18ull * nc + 2ull * (nc + 1) * MERGE_PAGE_BOUND / MERGE_RPS + 64; }
+
+/* The row rule over rows laid out span by span (span s at rows [span_row0[s], span_row0[s + 1]) of R), shared by the merge and the
+ * flush (flush.cu):
+ *   sort_spans          StableSortPairs by time inside each span: perm[i] = laid-out row of sorted row i (equal times keep their order)
+ *   find_runs           k_merge_heads (row_file[perm[i]] repeated inside a run: M_REPEAT into *d_err), the exclusive scan of the
+ *                       heads and each span's first output row (head, oidx, out_begin taken from `b`)
+ *   combine_and_encode  k_merge_combine into 1000-row segment slots (each column takes its last non-null value in sorted order),
+ *                       then encode_columns; ns gets the batch, seg_first[k] the first segment of span k in it ([n_spans + 1]).
+ *                       span_has (may be null): [span][column] set where the column holds a value in the span. */
+struct SortedRows {
+    const int64_t *t; const uint32_t *perm, *row_span, *span_row0; /* row_span: by sorted position */
+    const uint64_t *cells; const uint8_t *ok;                      /* [column][laid-out row] */
+    uint32_t R, n_spans;
+    uint32_t *head = nullptr, *oidx = nullptr, *out_begin = nullptr;
+};
+int sort_spans(const int64_t *times, int64_t *times_sorted, uint32_t *perm_in, uint32_t *perm, uint32_t R, uint32_t n_spans,
+               const uint32_t *d_span_row0, Scratch &b);
+int find_runs(SortedRows &r, const uint32_t *row_file, Scratch &b, MergeErr *d_err);
+int combine_and_encode(const SortedRows &r, const std::vector<int32_t> &types, const int32_t *d_types, Scratch &b, unsigned long long *d_rep,
+                       uint8_t *span_has, Scratch &blobs, NewSegs &ns, std::vector<uint32_t> &seg_first);
+
+/* per probed series: its last time, and the range [a, b) of its segments that a span [lo, hi] overlaps (merge.cu) */
+__global__ void k_append_probe(const uint32_t *series_seg_begin, const int64_t *seg_tmin, const int64_t *seg_tmax, const uint32_t *series,
+                               const int64_t *lo, const int64_t *hi, uint32_t n, int64_t *last, uint32_t *a_out, uint32_t *b_out);
+
+/* New files whose pages are already on the device, as the flush (flush.cu) produces them: file f's pages at data + base[f], where
+ * build_file_dir places a file set (16-byte aligned, back to back), followed by 1024 zero bytes; rows[] the rows of every segment,
+ * files in order.  add_files takes the region over instead of copying host files in; the encoders wrote the pages, so they are
+ * not validated again. */
+struct DeviceFiles {
+    uint8_t *data = nullptr; uint64_t data_len = 0;
+    std::vector<uint32_t> rows;
+    DeviceFiles() = default;
+    DeviceFiles(const DeviceFiles &) = delete;
+    DeviceFiles &operator=(const DeviceFiles &) = delete;
+    ~DeviceFiles() { dev_free(data); }
+};
+/* files[] join `s` (og_shard_append_files; og_shard_open_files on an empty shard).  `who` names the caller in refusals.  dev: the
+ * files' pages are on the device already (files[f].data is then never read) */
+int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, const char *who, DeviceFiles *dev);
+
 /* the refusal of a string value inside a span `pass` re-encodes, or of a page that failed to decode in segment `seg` of `where` */
 int string_refusal(unsigned long long sid, const std::string &column, const char *pass);
 int decode_failure(int device_code, uint32_t seg, const char *where);

@@ -135,6 +135,86 @@ class Shard:
         self._with_file_descs(files, call)
         return self
 
+    @staticmethod
+    def colval(typ, values, valid, bitmap_offset=0, bitmap=True):
+        """One column of a flush in the ColVal layout (lib/record/column.go): values / valid per row -> a dict of the pieces
+        rows_desc takes, the non-null values packed densely, the bitmap LSB-first from bit bitmap_offset (bitmap=False: no
+        bitmap, which the library accepts only when no row is null)."""
+        valid = np.asarray(valid, bool)
+        n = valid.size
+        dt = "<u1" if typ == L.TYPE_BOOL else "<f8" if typ == L.TYPE_FLOAT else "<i8"
+        dense = np.ascontiguousarray(np.asarray(values)[valid], dtype=dt)
+        bm = None
+        if bitmap:
+            bits = np.concatenate([np.zeros(bitmap_offset, np.uint8), valid.astype(np.uint8)])
+            bm = np.packbits(bits, bitorder="little") if bits.size else np.zeros(1, np.uint8)
+        return dict(type=typ, val=dense.view(np.uint8), bitmap=bm, bitmap_offset=bitmap_offset, len=n, nil_count=int(n - valid.sum()))
+
+    @staticmethod
+    def rows_desc(fields, series, flags=0):
+        """An L.RowsDesc (og_rows_desc) over explicit ColVal pieces.  fields: [(name, type)]; series: [(sid, times, cols)] with
+        cols[f] a Shard.colval dict (its keys may be overridden) or None for a column the series lacks (len 0)."""
+        keep = []
+        fs = (L.RowsField * max(1, len(fields)))()
+        for i, (name, typ) in enumerate(fields):
+            fs[i].name, fs[i].type = name.encode(), typ
+        ss = (L.RowsSeries * max(1, len(series)))()
+        for k, (sid, times, cols) in enumerate(series):
+            t = np.ascontiguousarray(times, dtype=np.int64)
+            cv = (L.ColValView * max(1, len(fields)))()
+            keep += [t, cv]
+            for f, c in enumerate(cols):
+                if c is None:
+                    continue
+                val = np.ascontiguousarray(c["val"], dtype=np.uint8)
+                keep.append(val)
+                cv[f].val = _ptr(val, C.c_uint8) if val.size else None
+                cv[f].val_bytes = c.get("val_bytes", val.size)
+                if c.get("bitmap") is not None:
+                    bm = np.ascontiguousarray(c["bitmap"], dtype=np.uint8)
+                    keep.append(bm)
+                    cv[f].bitmap = _ptr(bm, C.c_uint8)
+                cv[f].type, cv[f].len, cv[f].nil_count, cv[f].bitmap_offset = c["type"], c["len"], c["nil_count"], c["bitmap_offset"]
+            ss[k].sid, ss[k].rows, ss[k].times, ss[k].cols = sid, t.size, _ptr(t, C.c_int64), cv
+        d = L.RowsDesc(len(fields), fs, len(series), ss, flags)
+        d._keep = (keep, fs, ss)
+        return d
+
+    @classmethod
+    def batch_desc(cls, batch):
+        """{sid: {"times", "cols": {name: (type, values per row, valid per row)}}} -> L.RowsDesc, fields sorted by name, a column
+        a series lacks passed with len 0"""
+        types = {n: t for s_ in batch.values() for n, (t, _v, _k) in s_["cols"].items()}
+        names = sorted(types)
+        series = [(sid, s_["times"], [cls.colval(*s_["cols"][n]) if n in s_["cols"] else None for n in names]) for sid, s_ in batch.items()]
+        return cls.rows_desc([(n, types[n]) for n in names], series)
+
+    @staticmethod
+    def _rows_info(info):
+        out = {k: getattr(info, k) for k, _ in L.RowsInfo._fields_ if k != "phase_ms"}
+        out["phase_ms"] = list(info.phase_ms)
+        return out
+
+    def append_rows(self, batch):
+        """Flush rows into the shard (og_shard_append_rows): batch is a {sid: {"times", "cols"}} dict (batch_desc) or an
+        L.RowsDesc (rows_desc).  Rows are sorted and deduplicated per series, split at the series' last time in the shard into
+        an ordered and an out-of-order file, encoded and appended on the device.  Returns the og_rows_info counters."""
+        d = batch if isinstance(batch, L.RowsDesc) else self.batch_desc(batch)
+        info = L.RowsInfo()
+        L.check(L.lib().og_shard_append_rows(self.h, C.byref(d), C.byref(info)), "og_shard_append_rows")
+        return self._rows_info(info)
+
+    @classmethod
+    def open_rows(cls, batch):
+        """A new shard from one flush (og_shard_open_rows); batch as append_rows takes it.  The counters are sh.rows_info."""
+        d = batch if isinstance(batch, L.RowsDesc) else cls.batch_desc(batch)
+        info = L.RowsInfo()
+        h = C.c_void_p()
+        L.check(L.lib().og_shard_open_rows(C.byref(d), C.byref(h), C.byref(info)), "og_shard_open_rows")
+        sh = cls(h.value)
+        sh.rows_info = cls._rows_info(info)
+        return sh
+
     def compact(self, rows_per_segment=0):
         """Re-cut every series into full segments of rows_per_segment rows (0: 1000), the last one 1..rows_per_segment, every
         column of a series with a page in each (og_shard_compact).  Returns the og_compact_info counters as a dict; all zero when
