@@ -7,7 +7,9 @@ compacted shard must hold.
        - else at the first segment that is not the last and holds fewer than R rows, or holds more than R
   2. the rows from there on decoded with oracle.time_page_decode / field_page_decode (null where a segment has no page)
   3. cut into segments of R rows, the remainder last; every column of the series gets a page in each, from the oracle's encoders
-     (a float segment the Gorilla encoder refuses, +Inf and -Inf in one segment, gets the raw page [header][0x00][values LE]);
+     (a float segment the Gorilla encoder refuses, +Inf and -Inf in one segment, gets the raw page [header][0x00][values LE], and
+     an int segment the reference would hand to zstd, a zig-zag delta above 2^60 - 1, the raw page [header][0x40][u32 BE 8n][zig-zag
+     BE values], int.go uncompressedData);
      a string column, which must be null in every re-cut row, gets the all-null page [44][u32 BE rows]
 
 The device encoders write a raw page where the reference takes Snappy (NaN, few decimals: DESIGN.md "Deviations"), so byte
@@ -62,15 +64,29 @@ def raw_float_page(values, valid):
     return np.frombuffer(_header(L.TYPE_FLOAT, valid) + b"\x00" + np.ascontiguousarray(values[valid], "<f8").tobytes(), np.uint8)
 
 
+def zigzag_be(values):
+    """int64 values -> their zig-zag encodings as big-endian bytes (MarshalInt64Append)"""
+    v = np.asarray(values, np.int64)
+    return ((v.astype(np.uint64) << np.uint64(1)) ^ (v >> np.int64(63)).astype(np.uint64)).astype(">u8").tobytes()
+
+
+def raw_int_page(values, valid):
+    """the encoders' raw page for an int segment: header, 0x40, u32 BE 8n, the non-null values zig-zag big-endian"""
+    v = np.asarray(values, np.int64)[valid]
+    return np.frombuffer(_header(L.TYPE_INT, valid) + struct.pack(">BI", 0x40, 8 * v.size) + zigzag_be(v), np.uint8)
+
+
 def encode_field(typ, values, valid):
     if typ == TYPE_STRING:
         return np.frombuffer(bytes([44]) + struct.pack(">I", valid.size), np.uint8)
     try:
         return oracle.field_page_encode(typ, np.ascontiguousarray(values), None if valid.all() else valid.astype(np.uint8))
     except ValueError:
-        if typ != L.TYPE_FLOAT:
-            raise
-        return raw_float_page(values, valid)
+        if typ == L.TYPE_FLOAT:
+            return raw_float_page(values, valid)
+        if typ == L.TYPE_INT:  # the oracle does not restate zstd: the device writes the raw block there
+            return raw_int_page(values, valid)
+        raise
 
 
 def _page(ex, c, g):

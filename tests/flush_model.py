@@ -5,7 +5,9 @@ for one batch of rows.
      sorted stably by time; for a run of equal times each column takes the last non-null value in arrival order, a null never
      replaces a value (replace, :100-107)
   2. split at the series' last time in the shard (SplitRecordByTime, engine/mutable/ts_table.go:242-290): t > last ordered,
-     t <= last out of order; a column with no non-null value in a part is left out of that part (:276-286)
+     t <= last out of order; a column with no non-null value in a part is left out of that part (:276-286), also when every row
+     falls into one part, where the reference hands the record on unchanged and keeps such a column (:243-248; DESIGN.md
+     "Deviations")
   3. each part is one series of a file; file_desc cuts it into 1000-row segments from its first row (WriteData), every kept
      column with a page in each, pages from compact_model.encode_field (raw page where Gorilla refuses a float segment)
 

@@ -115,6 +115,22 @@ def test_raw_float_page_restates_the_encoders():
     assert np.array_equal(dok, ok) and np.array_equal(dv, v[ok])
 
 
+def test_raw_int_page_where_the_reference_takes_zstd():
+    """a zig-zag delta above 2^60 - 1: the oracle does not restate zstd, encode_field writes the uncompressed block"""
+    v = np.array([0, 1 << 59, 3, -(1 << 62), (1 << 63) - 1, -(1 << 63)], np.int64)
+    ok = np.array([1, 1, 0, 1, 1, 1], bool)
+    with pytest.raises(ValueError):
+        oracle.field_page_encode(L.TYPE_INT, v, ok.astype(np.uint8))
+    p = cm.encode_field(L.TYPE_INT, v, ok)
+    assert np.array_equal(p, cm.raw_int_page(v, ok))
+    nb = 1  # [2][u32 1][bitmap][u32 0][u32 1][0x40][u32 40][zig-zag BE x 5]
+    assert p[0] == L.TYPE_INT and p[13 + nb] == 0x40 and int.from_bytes(p[14 + nb:18 + nb].tobytes(), "big") == 8 * 5
+    dv, dok = oracle.field_page_decode(L.TYPE_INT, p, cap=16)
+    assert np.array_equal(dok, ok) and np.array_equal(dv, v[ok])
+    full = cm.encode_field(L.TYPE_INT, v, np.ones(6, bool))
+    assert full[0] == 32 and np.array_equal(oracle.field_page_decode(L.TYPE_INT, full, cap=16)[0], v)
+
+
 # ---------------------------------------------------------------- ABI
 def test_compact_structs_match_the_header(tmp_path):
     pairs = {"og_compact_desc": L.CompactDesc, "og_compact_info": L.CompactInfo}

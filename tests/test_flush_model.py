@@ -81,6 +81,17 @@ def test_split_record_by_time_drops_an_all_null_column():
     assert sorted(order[1]) == ["a1"] and sorted(unorder[1]) == ["a2"]  # Len() == 2: one field and the time column
 
 
+@pytest.mark.parametrize("last, side", [(0, 0), (8, 1)])
+def test_split_drops_an_all_null_column_when_every_row_is_on_one_side(last, side):
+    """the flush's documented deviation: ts_table.go:243-248 returns the record itself when every row falls on one side, so the
+    reference keeps a column null in every row; the flush drops it there too, as it does when the rows straddle the last time"""
+    t = np.array([1, 2, 3, 7, 8], np.int64)
+    cols = {"a1": (INT, np.arange(5), np.ones(5, bool)), "a2": (FLOAT, np.zeros(5), np.zeros(5, bool))}
+    parts = fm.split(t, cols, last)
+    assert parts[1 - side] is None
+    assert parts[side][0].tolist() == t.tolist() and sorted(parts[side][1]) == ["a1"]
+
+
 # ---------------------------------------------------------------- hand-worked
 def test_a_null_never_replaces_a_value_and_the_last_value_wins():
     t = np.array([10, 10, 10, 20, 10], np.int64)
