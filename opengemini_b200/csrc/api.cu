@@ -826,7 +826,8 @@ OG_API int og_query_run(og_query *q) {
     CU(cudaMemsetAsync(q->d_err, 0, 64, st));
     CU(cudaEventRecord(q->ev0, st));
     const bool per_series = q->desc.group_mode == OG_GROUP_PER_SERIES;
-    if (!per_series) { k_init_dense<<<(unsigned)((cells_dense + 255) / 256), 256, 0, st>>>(p, gp); launches++; } /* per-series: k_merge_per_series writes every cell */
+    /* per-series: k_merge_per_series writes every cell of a series row; a shard without series still answers with one empty row */
+    if (!per_series || s->n_series == 0) { k_init_dense<<<(unsigned)((cells_dense + 255) / 256), 256, 0, st>>>(p, gp); launches++; }
     /* folded runs touch the per-series cells only on fallback paths: their validity bytes are cleared only after a run that used them */
     const bool clear_cells = !pl->fold || q->cells_dirty || n_chunks > 1;
     uint64_t segs_scanned = 0; uint32_t ci = 0, chunks_run = 0;

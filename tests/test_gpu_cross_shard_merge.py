@@ -32,6 +32,7 @@ import oracle
 import segment_shards as ss
 from opengemini_b200 import AggQuery, Comm, Shard
 from opengemini_b200 import _lib as L
+from records_model import assert_records, records_of
 
 pytestmark = pytest.mark.gpu
 
@@ -439,38 +440,6 @@ def test_chain_of_three_shards(mapped):
     a.close(); b.close(); c.close()
 
 
-def _records_of(d, calls, ascending, chunk):
-    """what og_query_next returns for dense record d: per tagset, slices of `chunk` windows (latest first when descending)
-    without their empty windows; a row's time is the window start (0 without an interval) or, for a single-call selector,
-    the selected point's time; multi-call first / last carry RecMeta.Times"""
-    nb, multi = d["n_buckets"], len(calls) > 1
-    out = []
-    for g in range(d["n_groups"]):
-        for s in range(0, nb, chunk):
-            rows = []
-            for b in range(s, min(nb, s + chunk)):
-                i = g * nb + (b if ascending else nb - 1 - b)
-                if any(c["valid"][i] for c in d["cols"]):
-                    rows.append((i, i - g * nb))
-            if not rows:
-                continue
-            times, cols = [], []
-            for i, bb in rows:
-                t = d["start"] + bb * d["interval"]
-                for (f, _c), c in zip(calls, d["cols"]):
-                    if c["times"] is not None and not multi and c["valid"][i]:
-                        t = int(c["times"][i])
-                times.append(t)
-            for (f, col), c in zip(calls, d["cols"]):
-                idx = np.array([i for i, _ in rows])
-                ok = np.asarray(c["valid"])[idx] != 0
-                v = np.asarray(c["values"]).view(np.uint64)[idx][ok]
-                ct = np.where(ok, np.asarray(c["times"])[idx], 0) if multi and c["times"] is not None else None
-                cols.append((ok, v, ct))
-            out.append((g, np.array(times, np.int64), cols))
-    return out
-
-
 @pytest.mark.parametrize("ascending", [True, False], ids=["asc", "desc"])
 def test_records_after_a_merge(ascending):
     """A <- B under the map; og_query_next runs once before the merge (the host copy of A's record is filled), then the records
@@ -488,18 +457,7 @@ def test_records_after_a_merge(ascending):
             _merge(qa, qb)
             got = qa.dense_host()
             _check(got, [a, b], [qa.desc, qb.desc], calls, q, label, True, sd)
-            want = _records_of(got, calls, ascending, 7)
-            recs = list(qa.records())
-            assert len(recs) == len(want), label
-            for r, (g, times, cols) in zip(recs, want):
-                assert r["group"] == g and np.array_equal(r["times"], times), label
-                for k, (rc, (ok, v, ct)) in enumerate(zip(r["cols"], cols)):
-                    assert np.array_equal(rc["valid"], ok), f"{label} col {k}: validity"
-                    rv = rc["values"].astype(np.uint64) if rc["type"] == L.TYPE_BOOL else rc["values"].view(np.uint64)
-                    assert np.array_equal(rv, v), f"{label} col {k}: values"
-                    assert (rc["times"] is None) == (ct is None), f"{label} col {k}: times presence"
-                    if ct is not None:
-                        assert np.array_equal(rc["times"], ct), f"{label} col {k}: times"
+            assert_records(list(qa.records()), records_of(got, calls, ascending, 7), label)
             qa.close(); qb.close()
     a.close(); b.close()
 
