@@ -39,7 +39,7 @@ cudaError_t dev_mem_info(size_t *free_b, size_t *total_b) {
     return cudaSuccess;
 }
 
-static int map_dev_err(int code) {
+int map_dev_err(int code) {
     switch (code) {
     case D_UNSUPPORTED: return OG_E_UNSUPPORTED;
     case D_TYPE: return OG_E_TYPE;
@@ -557,8 +557,8 @@ int ensure_il(og_shard *s, int col, cudaStream_t st) {
     if (n_dom64 >= (1ull << 31)) return OG_OK;
     const uint32_t n_dom = (uint32_t)n_dom64;
     int rc;
-    struct Ev { cudaEvent_t e = nullptr; Ev() { cudaEventCreate(&e); } ~Ev() { if (e) cudaEventDestroy(e); } } ev0, ev1;
-    cudaEventRecord(ev0.e, st);
+    EventTimer timer(st);
+    timer.start();
     Scratch tmp(st); /* k_il_scan and the sort may still run on st when a check below returns */
     IlScanOut so{};
     uint32_t *seg_words; uint64_t *keys2; uint32_t *vals2;
@@ -638,10 +638,10 @@ int ensure_il(og_shard *s, int col, cudaStream_t st) {
     CU(cudaMemcpyAsync(ic.grp_off, go.data(), (size_t)ng * 8, cudaMemcpyHostToDevice, st));
     k_il_repack<<<(unsigned)((n_slots + 127) / 128), 128, 0, st>>>(d, col, ic.lane_seg, ic.lane_win, ic.grp_off, ic.grp_rows, ng, ic.words);
     CU(cudaGetLastError());
-    cudaEventRecord(ev1.e, st);
+    timer.stop();
     CU(cudaStreamSynchronize(st));
-    float ms = 0; cudaEventElapsedTime(&ms, ev0.e, ev1.e);
-    ic.n_words = total; ic.n_packed = n_packed; ic.build_ms = ms; ic.state = 1;
+    timer.ms(&ic.build_ms);
+    ic.n_words = total; ic.n_packed = n_packed; ic.state = 1;
     return OG_OK;
 }
 

@@ -18,7 +18,7 @@
  *          encode_columns     the encoders of og_encode_pages, raw page for a float segment Gorilla refuses; string columns
  *                             (null in every re-cut row) get an all-null page from k_compact_null_pages
  *   finish the new directory from runs of the shard's kept segments and the new ones (splice_and_gather), the live pages gathered
- *          into a new data region, k_append_stats for the totals, and the new state swapped in whole.
+ *          into a new data region, k_append_stats for the totals, and install_state swaps the new state in whole.
  */
 #include <algorithm>
 #include <cstdio>
@@ -210,10 +210,7 @@ static int compact_spans(og_shard *s, uint32_t R, const std::vector<uint32_t> &r
                     else if (s->col_types[c] == OG_TYPE_STRING) { ns.off[pi] = nulls + 8ull * g; ns.len[pi] = 5; }
                 }
         }
-        ns.tmin.resize(NS); ns.tmax.resize(NS); ns.rows = h_rows;
-        CU(cudaMemcpy(ns.tmin.data(), d_tmin, NS * 8ull, cudaMemcpyDeviceToHost));
-        CU(cudaMemcpy(ns.tmax.data(), d_tmax, NS * 8ull, cudaMemcpyDeviceToHost));
-        if ((rc = keep_blob(blob, used, blobs, ns))) return rc;
+        if ((rc = keep_blob(d_tmin, d_tmax, std::move(h_rows), blob, used, blobs, ns))) return rc;
         batches.push_back(std::move(ns));
         a = b;
     }
@@ -252,35 +249,19 @@ static int compact(og_shard *s, uint32_t R, og_compact_info &info) {
         spans.push_back(sp);
     }
     if (spans.empty()) return OG_OK; /* already compact: nothing is copied */
-    /* the interleaved copies describe the old layout: dropped now (their memory serves the pass), rebuilt on first use */
-    {
-        std::lock_guard<std::mutex> il_lock(s->il_mu);
-        for (og_shard::IlCol &c : s->il)
-            dev_free_all(c.words, c.grp_off, c.grp_rows, c.grp_col, c.lane_seg, c.lane_rows, c.lane_series, c.lane_win, c.lane_t0, c.lane_dt, c.gen_list);
-        s->il.assign(s->n_columns, og_shard::IlCol{});
-    }
-    cudaEvent_t ev0, ev1;
-    CU(cudaEventCreate(&ev0)); CU(cudaEventCreate(&ev1));
-    struct FreeEv { cudaEvent_t a, b; ~FreeEv() { cudaEventDestroy(a); cudaEventDestroy(b); } } free_ev{ev0, ev1};
-    CU(cudaEventRecord(ev0, 0));
+    s->reset_il(); /* the copies describe the old layout: their memory serves the pass */
+    EventTimer timer;
+    CU(timer.start());
     std::vector<NewSegs> batches;
     Scratch blobs;
     if ((rc = compact_spans(s, R, rows, spans, batches, blobs))) return rc;
     /* ---- the new segments as one source, the shard's own as another ---- */
-    Scratch maps;
-    int32_t *d_identity;
-    if ((rc = maps.get(&d_identity, nc))) return rc;
-    {
-        std::vector<int32_t> identity(nc);
-        for (uint32_t c = 0; c < nc; c++) identity[c] = (int32_t)c;
-        CU(cudaMemcpy(d_identity, identity.data(), nc * 4ull, cudaMemcpyHostToDevice));
-    }
     SegSrc src[3] = {};
-    src[SRC_SHARD] = SegSrc{s->d_page_off, s->d_page_len, s->d_seg_rows, s->d_tmin, s->d_tmax, nullptr, 0, d_identity, NSEG, nc};
+    src[SRC_SHARD] = SegSrc{s->d_page_off, s->d_page_len, s->d_seg_rows, s->d_tmin, s->d_tmax, nullptr, 0, nullptr, NSEG, nc};
     std::vector<const uint8_t *> regions = {s->d_data, nullptr}; /* region 1 (files) is not used here */
     std::vector<uint32_t> m_first;
     Scratch m_own;
-    if ((rc = batches_source(batches, nc, d_identity, 2, regions, m_own, src[SRC_MERGED], m_first))) return rc;
+    if ((rc = batches_source(batches, nc, 2, regions, m_own, src[SRC_MERGED], m_first))) return rc;
     /* ---- the new directory as runs: per series its kept segments, then its new ones ---- */
     std::vector<Run> runs;
     std::vector<uint32_t> o_ssb(NSER + 1, 0);
@@ -303,28 +284,13 @@ static int compact(og_shard *s, uint32_t R, og_compact_info &info) {
     Scratch out_own;
     Spliced sd;
     if ((rc = splice_and_gather(src, runs, NOUT, nc, regions, out_own, sd))) return rc;
-    CU(cudaEventRecord(ev1, 0));
+    CU(timer.stop());
     if ((rc = spliced_totals(sd, nc, *out, "compaction"))) return rc;
     /* the Snappy counters hold while every transcoded page is in the shard: a re-cut drops them, as a merge does */
     out->rows_merged = true;
-    /* ---- the new state, complete and synchronised before it is swapped in: nothing fails after the swap ---- */
-    out->device = s->device; out->n_series = NSER; out->n_segments = NOUT; out->n_columns = nc;
-    out->sids = s->sids; out->col_types = s->col_types; out->col_names = s->col_names; out->h_series_seg_begin = o_ssb;
     out->merge = s->merge;
-    if ((rc = dalloc(&out->d_series_seg_begin, (size_t)NSER + 1)) || (rc = dalloc(&out->d_sids, (size_t)NSER))) return rc;
-    CU(cudaMemcpy(out->d_series_seg_begin, o_ssb.data(), ((size_t)NSER + 1) * 4, cudaMemcpyHostToDevice));
-    if (NSER) CU(cudaMemcpy(out->d_sids, s->sids.data(), (size_t)NSER * 8, cudaMemcpyHostToDevice));
-    float ms = 0;
-    CU(cudaEventElapsedTime(&ms, ev0, ev1));
-    info.compact_ms = ms;
-    take_spliced(out_own, sd, *out);
-    CU(cudaDeviceSynchronize());
-    std::swap(static_cast<ShardState &>(*s), static_cast<ShardState &>(*out));
-    {
-        std::lock_guard<std::mutex> il_lock(s->il_mu);
-        s->il.assign(s->n_columns, og_shard::IlCol{});
-    }
-    return OG_OK;
+    CU(timer.ms(&info.compact_ms));
+    return install_state(s, *out, out_own, sd, o_ssb, s->sids, s->col_types, s->col_names);
 }
 
 } // namespace ogpu
@@ -338,13 +304,12 @@ OG_API int og_shard_compact(og_shard *s, const og_compact_desc *d, og_compact_in
     if (d->flags) { set_error("og_compact_desc.flags must be 0 (got %u)", d->flags); return OG_E_INVAL; }
     if (d->rows_per_segment > 1000) { set_error("rows_per_segment must be 0 (1000) or 1..1000 (got %u)", d->rows_per_segment); return OG_E_INVAL; }
     const uint32_t R = d->rows_per_segment ? d->rows_per_segment : COMPACT_RPS_DEFAULT;
-    std::lock_guard<std::mutex> lock(s->live->mu); /* og_query_create waits until the compaction is done */
-    if (s->live->n) { set_error("%u queries on this shard are still open: destroy them before compacting it", s->live->n); return OG_E_STATE; }
-    CU(cudaSetDevice(s->device));
-    og_compact_info ci{};
-    const int rc = compact(s, R, ci);
-    if (rc == OG_OK && info) *info = ci;
-    return rc;
+    return rewrite_shard(s, "compacting it", [&] {
+        og_compact_info ci{};
+        const int rc = compact(s, R, ci);
+        if (rc == OG_OK && info) *info = ci;
+        return rc;
+    });
 }
 
 } // extern "C"

@@ -138,7 +138,6 @@ struct og_downsampled {
 static int downsample_pass(og_shard *s, int64_t interval, int64_t tmin, int64_t tmax, const std::vector<std::vector<og_call>> &qcalls,
                            const std::vector<OutCol> &oc, og_downsampled **out) {
     using clock = std::chrono::steady_clock;
-    auto ms_since = [](clock::time_point t0) { return std::chrono::duration<double, std::milli>(clock::now() - t0).count(); };
     CU(cudaSetDevice(s->device));
     const auto t_start = clock::now();
     const uint32_t n_oc = (uint32_t)oc.size(), ns = s->n_series;

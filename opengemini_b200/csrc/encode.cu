@@ -24,10 +24,6 @@
 
 namespace ogpu {
 
-int shard_finalize(og_shard *s, bool scan_snappy); /* api.cu */
-int alloc_dir(og_shard *s);                        /* api.cu */
-int ensure_device();              /* api.cu */
-
 #define PAGE_STRIDE 8704u /* staging bytes per page: worst case 13 + 125 + 1 + 8000 (raw) rounded up, 8-byte aligned */
 
 /* MSB-first bit writer with 8-byte aligned big-endian stores */

@@ -40,9 +40,6 @@
 
 namespace ogpu {
 
-int gather_pages(const std::vector<const uint8_t *> &regions, const std::vector<uint32_t> &page_region, const std::vector<uint64_t> &src_off,
-                 const std::vector<uint32_t> &len, const std::vector<uint64_t> &dst_off, uint8_t *out); /* merge.cu */
-
 /* one (series, column) of a batch: its values at stage + val_off (8 bytes each, 1 for bool), its bitmap bits from bit bit0 of
  * stage + bm_off (no bitmap: every row valid) */
 struct FlushTask { uint64_t val_off, bm_off; uint32_t row0, rows, col, bit0; };
@@ -99,10 +96,6 @@ __global__ void k_flush_row_span(const uint32_t *span_row0, uint32_t n_spans, ui
     uint32_t lo = 0, hi = n_spans;
     while (hi - lo > 1) { const uint32_t m = (lo + hi) / 2; if (span_row0[m] <= i) lo = m; else hi = m; }
     row_span[i] = lo;
-}
-
-static double ms_since(std::chrono::steady_clock::time_point t0) {
-    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
 }
 
 static uint64_t value_width(int32_t type) { return type == OG_TYPE_BOOL ? 1 : 8; }
@@ -184,19 +177,9 @@ static int flush_batches(const og_shard *s, const og_rows_desc *d, const std::ve
             auto it = old_of_sid.find(d->series[order[k]].sid);
             if (it != old_of_sid.end()) { pk.push_back(k); po.push_back(it->second); }
         }
-        const uint32_t NP = (uint32_t)pk.size();
-        if (NP) {
-            Scratch t;
-            uint32_t *d_ser, *d_a, *d_b; int64_t *d_lo, *d_last;
-            if ((rc = t.get(&d_ser, NP)) || (rc = t.get(&d_lo, NP)) || (rc = t.get(&d_last, NP)) || (rc = t.get(&d_a, NP)) || (rc = t.get(&d_b, NP))) return rc;
-            CU(cudaMemcpy(d_ser, po.data(), NP * 4ull, cudaMemcpyHostToDevice));
-            CU(cudaMemset(d_lo, 0, NP * 8ull));
-            k_append_probe<<<(NP + 127) / 128, 128>>>(s->d_series_seg_begin, s->d_tmin, s->d_tmax, d_ser, d_lo, d_lo, NP, d_last, d_a, d_b);
-            CU(cudaGetLastError());
-            std::vector<int64_t> h(NP);
-            CU(cudaMemcpy(h.data(), d_last, NP * 8ull, cudaMemcpyDeviceToHost));
-            for (uint32_t j = 0; j < NP; j++) last[pk[j]] = h[j];
-        }
+        Probe pr;
+        if ((rc = probe_series(s, po, nullptr, nullptr, pr))) return rc;
+        for (size_t j = 0; j < pk.size(); j++) last[pk[j]] = pr.last[j];
     }
     /* A batch's scratch follows its rows (staging, cells, sort) and its output slots (segment slots and encoder blob, per slot as
        much as span_row_bytes charges a row).  Every non-empty part takes whole 1000-row segments, so a series is charged its rows
@@ -441,22 +424,12 @@ extern "C" {
 
 OG_API int og_shard_append_rows(og_shard *s, const og_rows_desc *rows, og_rows_info *info) {
     if (!s || !rows) { set_error("null argument"); return OG_E_INVAL; }
-    std::lock_guard<std::mutex> lock(s->live->mu); /* og_query_create waits until the flush is done */
-    if (s->live->n) { set_error("%u queries on this shard are still open: destroy them before appending rows", s->live->n); return OG_E_STATE; }
-    CU(cudaSetDevice(s->device));
-    return flush_rows(s, rows, info, "og_shard_append_rows");
+    return rewrite_shard(s, "appending rows", [&] { return flush_rows(s, rows, info, "og_shard_append_rows"); });
 }
 
 OG_API int og_shard_open_rows(const og_rows_desc *rows, og_shard **out, og_rows_info *info) {
     if (!rows || !out) { set_error("null argument"); return OG_E_INVAL; }
-    *out = nullptr;
-    int rc = ensure_device(); if (rc) return rc;
-    std::unique_ptr<og_shard> s(new og_shard); /* a flush into an empty shard */
-    CU(cudaGetDevice(&s->device));
-    s->h_series_seg_begin = {0};
-    if ((rc = flush_rows(s.get(), rows, info, "og_shard_open_rows"))) return rc;
-    *out = s.release();
-    return OG_OK;
+    return open_empty(out, [&](og_shard *s) { return flush_rows(s, rows, info, "og_shard_open_rows"); });
 }
 
 } // extern "C"

@@ -4,6 +4,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <chrono>
 #include <cstdint>
 #include <memory>
 #include <string>
@@ -21,6 +22,39 @@ namespace ogpu {
 void set_error(const char *fmt, ...);
 int cuda_fail(cudaError_t e, const char *what, const char *file, int line);
 int ensure_device(); /* bind the calling thread to the library's device (og_init(0) on first use) */
+int map_dev_err(int device_code); /* a device decode code (decode.cuh D_*) as the OG_E_* status a call returns */
+
+inline double ms_since(std::chrono::steady_clock::time_point t0) {
+    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+}
+
+/* two events that time work on one stream: start() creates and records the first, stop() records the second, ms() is the time
+ * between them once the stop event has completed */
+struct EventTimer {
+    cudaStream_t stream;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    explicit EventTimer(cudaStream_t st = 0) : stream(st) {}
+    EventTimer(const EventTimer &) = delete;
+    EventTimer &operator=(const EventTimer &) = delete;
+    ~EventTimer() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+    cudaError_t start() {
+        for (cudaEvent_t &e : ev) { const cudaError_t r = cudaEventCreate(&e); if (r != cudaSuccess) return r; }
+        return cudaEventRecord(ev[0], stream);
+    }
+    cudaError_t stop() { return cudaEventRecord(ev[1], stream); }
+    cudaError_t ms(double *out) const { float m = 0; const cudaError_t e = cudaEventElapsedTime(&m, ev[0], ev[1]); *out = m; return e; }
+};
+
+/* api.cu: the steps of opening a shard */
+int check_desc(const og_shard_desc *d);
+int alloc_dir(og_shard *s);
+int upload_dir(og_shard *s, const uint32_t *series_seg_begin, const int64_t *seg_tmin, const int64_t *seg_tmax, const uint64_t *page_off,
+               const uint32_t *page_len, const uint64_t *sids);
+int shard_finalize(og_shard *s, bool scan_snappy);
+/* encode.cu: og_encode_pages; nan_raw: see encode_float_page */
+int encode_pages(int32_t type, int32_t is_time, const void *d_values, const uint8_t *d_valid, const uint32_t *d_rows, uint32_t n_segments,
+                 uint32_t rps, uint8_t *d_out, uint64_t out_cap, uint64_t *d_page_off, uint32_t *d_page_len, uint64_t *total_bytes_out,
+                 bool nan_raw);
 
 /* Device memory comes from the device's stream-ordered pool (cudaMallocAsync on the legacy stream) with its release threshold
  * raised at og_init: shards and queries that are opened and closed in a loop get their buffers back from the pool instead of
@@ -60,11 +94,12 @@ struct Scratch {
     template <class T> int get(T **p, size_t n) { int rc = dalloc(p, n); if (rc == OG_OK) bufs.push_back(*p); return rc; }
 };
 
-/* the live queries of a shard: og_query_create counts up, ~og_query down, og_shard_append_files holds `mu` throughout.  Shared by
- * the shard and its queries, so a query destroyed after its shard was closed still finds it. */
+/* the live queries of a shard: og_query_create counts up, ~og_query down, a rewrite of the shard (rewrite_shard, span_pass.h)
+ * holds `mu` throughout.  Shared by the shard and its queries, so a query destroyed after its shard was closed still finds it. */
 struct LiveQueries { std::mutex mu; uint32_t n = 0; };
 
-/* everything that describes a shard's rows and where they live: og_shard_append_files builds a new one and swaps it in whole */
+/* everything that describes a shard's rows and where they live: a rewrite builds a new one and install_state (span_pass.h) swaps
+ * it in whole */
 struct ShardState {
     int device = 0;
     uint8_t *d_data = nullptr; uint64_t data_len = 0; bool owns_data = true;
@@ -109,13 +144,20 @@ struct og_shard : ogpu::ShardState {
     std::vector<IlCol> il; /* [n_columns] */
     std::mutex il_mu;      /* queries of one shard may be planned from different threads: the build is serialised */
     std::shared_ptr<ogpu::LiveQueries> live = std::make_shared<ogpu::LiveQueries>();
+    /* every interleaved copy freed, one unbuilt entry per column left: a rewrite of the shard drops the copies of the old layout,
+     * and the first query that wants one builds it again */
+    void reset_il() {
+        std::lock_guard<std::mutex> lock(il_mu);
+        for (IlCol &c : il)
+            ogpu::dev_free_all(c.words, c.grp_off, c.grp_rows, c.grp_col, c.lane_seg, c.lane_rows, c.lane_series, c.lane_win, c.lane_t0, c.lane_dt, c.gen_list);
+        il.assign(n_columns, IlCol{});
+    }
     ~og_shard() {
         using ogpu::dev_free_all;
         if (owns_data) dev_free_all(d_data);
         dev_free_all(d_series_seg_begin, d_seg_series, d_seg_rows, d_tmin, d_tmax, d_page_off, d_page_len, d_sids, d_seg_buf);
         if (h_seg_buf) cudaFreeHost(h_seg_buf);
-        for (IlCol &c : il)
-            dev_free_all(c.words, c.grp_off, c.grp_rows, c.grp_col, c.lane_seg, c.lane_rows, c.lane_series, c.lane_win, c.lane_t0, c.lane_dt, c.gen_list);
+        reset_il();
     }
 };
 

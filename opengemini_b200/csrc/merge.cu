@@ -31,7 +31,7 @@
  *   finish k_append_splice builds the new directory from runs of the shard's, the files' and the merge's segments; k_append_gather
  *          copies the live pages into a new data region, unless the files' region already holds every one of them (nothing merged
  *          and no older segments), which is then kept as it is; k_append_stats derives the shard's totals from the time pages'
- *          headers, and the new state is swapped in whole.
+ *          headers, and install_state swaps the new state in whole.
  *
  * The gather's copy loop is not shared with k_tssp_gather: the writer's CRC needs each lane to own one contiguous slice of a page,
  * the gather deals 16-byte blocks out across the lanes so that a warp's loads and stores are consecutive.
@@ -52,15 +52,6 @@
 #include "span_pass.h"
 
 namespace ogpu {
-
-int shard_finalize(og_shard *s, bool scan_snappy); /* api.cu */
-int check_desc(const og_shard_desc *d);            /* api.cu */
-int upload_dir(og_shard *s, const uint32_t *series_seg_begin, const int64_t *seg_tmin, const int64_t *seg_tmax, const uint64_t *page_off,
-               const uint32_t *page_len, const uint64_t *sids); /* api.cu */
-int encode_pages(int32_t type, int32_t is_time, const void *d_values, const uint8_t *d_valid, const uint32_t *d_rows, uint32_t n_segments,
-                 uint32_t rps, uint8_t *d_out, uint64_t out_cap, uint64_t *d_page_off, uint32_t *d_page_len, uint64_t *total_bytes_out,
-                 bool nan_raw); /* encode.cu */
-
 
 __device__ __forceinline__ bool merge_claim(MergeErr *e, int code) { return atomicCAS(&e->code, 0, code) == 0; }
 
@@ -227,11 +218,7 @@ int combine_and_encode(const SortedRows &r, const std::vector<int32_t> &types, c
     if ((rc = b.get(&blob, cap))) return rc;
     uint64_t used = 0;
     if ((rc = encode_columns(types, out_t, h_cols, out_ok, out_rows, d_rows, NS, MERGE_RPS, blob, cap, ns, &used))) return rc;
-    ns.tmin.resize(NS); ns.tmax.resize(NS); ns.rows = h_rows;
-    CU(cudaMemcpy(ns.tmin.data(), d_tmin, NS * 8ull, cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(ns.tmax.data(), d_tmax, NS * 8ull, cudaMemcpyDeviceToHost));
-    /* keep only the bytes written: the batch's scratch goes back to the pool before the next batch */
-    return keep_blob(blob, used, blobs, ns);
+    return keep_blob(d_tmin, d_tmax, std::move(h_rows), blob, used, blobs, ns);
 }
 
 /* Merge every span on the device, batch by batch: the spans' source segments are read through `dir`, whose columns are `types` /
@@ -500,7 +487,7 @@ __global__ void k_append_splice(SpliceP p) {
     p.tmin[g] = S.tmin[i]; p.tmax[g] = S.tmax[i]; p.rows[g] = S.rows[i]; p.series[g] = r.series;
     p.region[g] = S.seg_region ? S.seg_region[i] : S.region;
     for (uint32_t c = 0; c <= p.n_columns; c++) {
-        const int sc = c == p.n_columns ? (int)S.n_columns : S.col[c];
+        const int sc = c == p.n_columns ? (int)S.n_columns : S.col ? S.col[c] : (int)c;
         const size_t o = (size_t)c * p.n_out + g;
         if (sc < 0) { p.off[o] = 0; p.len[o] = 0; continue; }
         const size_t pi = (size_t)sc * S.n_segments + i;
@@ -543,8 +530,6 @@ __global__ void __launch_bounds__(APPEND_GATHER_THREADS) k_append_gather(const u
     for (uint32_t i = tail + lane; i < l; i += 32) dst[i] = __ldg(src + i);
 }
 
-/* pages from regions[page_region[p]] + src_off[p] to out + dst_off[p] (len[p] bytes each) with k_append_gather: the flush's
- * pages into the region of its files (flush.cu) */
 int gather_pages(const std::vector<const uint8_t *> &regions, const std::vector<uint32_t> &page_region, const std::vector<uint64_t> &src_off,
                  const std::vector<uint32_t> &len, const std::vector<uint64_t> &dst_off, uint8_t *out) {
     int rc;
@@ -566,8 +551,8 @@ int gather_pages(const std::vector<const uint8_t *> &regions, const std::vector<
 }
 
 /* per probed series of the shard: its last time, and the range [a, b) of its segments that a span [lo, hi] overlaps */
-__global__ void k_append_probe(const uint32_t *series_seg_begin, const int64_t *seg_tmin, const int64_t *seg_tmax, const uint32_t *series,
-                               const int64_t *lo, const int64_t *hi, uint32_t n, int64_t *last, uint32_t *a_out, uint32_t *b_out) {
+static __global__ void k_append_probe(const uint32_t *series_seg_begin, const int64_t *seg_tmin, const int64_t *seg_tmax, const uint32_t *series,
+                                      const int64_t *lo, const int64_t *hi, uint32_t n, int64_t *last, uint32_t *a_out, uint32_t *b_out) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n) return;
     const uint32_t g0 = series_seg_begin[series[k]], g1 = series_seg_begin[series[k] + 1];
@@ -577,6 +562,32 @@ __global__ void k_append_probe(const uint32_t *series_seg_begin, const int64_t *
     uint32_t b = a; e = g1;   /* first segment from a with tmin > hi */
     while (b < e) { const uint32_t m = (b + e) / 2; if (seg_tmin[m] <= hi[k]) b = m + 1; else e = m; }
     a_out[k] = a - g0; b_out[k] = b - g0;
+}
+
+int probe_series(const og_shard *s, const std::vector<uint32_t> &series, const int64_t *lo, const int64_t *hi, Probe &out) {
+    int rc;
+    const uint32_t n = (uint32_t)series.size();
+    out.last.assign(n, INT64_MIN); out.a.clear(); out.b.clear();
+    if (!n) return OG_OK;
+    Scratch t;
+    uint32_t *d_ser, *d_a, *d_b; int64_t *d_lo, *d_hi, *d_last;
+    if ((rc = t.get(&d_ser, n)) || (rc = t.get(&d_lo, n)) || (rc = t.get(&d_hi, n)) || (rc = t.get(&d_last, n)) || (rc = t.get(&d_a, n)) || (rc = t.get(&d_b, n))) return rc;
+    CU(cudaMemcpy(d_ser, series.data(), n * 4ull, cudaMemcpyHostToDevice));
+    if (lo) {
+        CU(cudaMemcpy(d_lo, lo, n * 8ull, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(d_hi, hi, n * 8ull, cudaMemcpyHostToDevice));
+    } else {
+        CU(cudaMemset(d_lo, 0, n * 8ull)); CU(cudaMemset(d_hi, 0, n * 8ull));
+    }
+    k_append_probe<<<(n + 127) / 128, 128>>>(s->d_series_seg_begin, s->d_tmin, s->d_tmax, d_ser, d_lo, d_hi, n, d_last, d_a, d_b);
+    CU(cudaGetLastError());
+    CU(cudaMemcpy(out.last.data(), d_last, n * 8ull, cudaMemcpyDeviceToHost));
+    if (lo) {
+        out.a.resize(n); out.b.resize(n);
+        CU(cudaMemcpy(out.a.data(), d_a, n * 4ull, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(out.b.data(), d_b, n * 4ull, cudaMemcpyDeviceToHost));
+    }
+    return OG_OK;
 }
 
 /* the derived totals of a spliced directory: rows, page bytes, time pages that are neither const-delta nor one-row, the largest
@@ -682,8 +693,12 @@ int encode_columns(const std::vector<int32_t> &types, const int64_t *d_times, co
     return OG_OK;
 }
 
-int keep_blob(const uint8_t *blob, uint64_t used, Scratch &blobs, NewSegs &ns) {
+int keep_blob(const int64_t *d_tmin, const int64_t *d_tmax, std::vector<uint32_t> rows, const uint8_t *blob, uint64_t used, Scratch &blobs,
+              NewSegs &ns) {
     int rc;
+    ns.tmin.resize(ns.n); ns.tmax.resize(ns.n); ns.rows = std::move(rows);
+    CU(cudaMemcpy(ns.tmin.data(), d_tmin, ns.n * 8ull, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(ns.tmax.data(), d_tmax, ns.n * 8ull, cudaMemcpyDeviceToHost));
     if ((rc = blobs.get(&ns.blob, used + 1024))) return rc;
     if (used) CU(cudaMemcpy(ns.blob, blob, used, cudaMemcpyDeviceToDevice));
     CU(cudaMemset(ns.blob + used, 0, 1024));
@@ -698,11 +713,11 @@ int string_refusal(unsigned long long sid, const std::string &column, const char
 
 int decode_failure(int device_code, uint32_t seg, const char *where) {
     set_error("segment %u of the %s failed to decode (device code %d)", seg, where, device_code);
-    return device_code == D_UNSUPPORTED ? OG_E_UNSUPPORTED : OG_E_CORRUPT;
+    return map_dev_err(device_code);
 }
 
-int batches_source(const std::vector<NewSegs> &batches, uint32_t nc, const int32_t *d_identity, uint32_t first_region,
-                   std::vector<const uint8_t *> &regions, Scratch &own, SegSrc &out, std::vector<uint32_t> &m_first) {
+int batches_source(const std::vector<NewSegs> &batches, uint32_t nc, uint32_t first_region, std::vector<const uint8_t *> &regions,
+                   Scratch &own, SegSrc &out, std::vector<uint32_t> &m_first) {
     int rc;
     m_first.assign(batches.size() + 1, 0);
     for (size_t b = 0; b < batches.size(); b++) m_first[b + 1] = m_first[b] + batches[b].n;
@@ -729,7 +744,7 @@ int batches_source(const std::vector<NewSegs> &batches, uint32_t nc, const int32
     CU(cudaMemcpy(d_reg, reg.data(), NM * 4ull, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(d_tmin, tmin.data(), NM * 8ull, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(d_tmax, tmax.data(), NM * 8ull, cudaMemcpyHostToDevice));
-    out = SegSrc{d_off, d_len, d_rows, d_tmin, d_tmax, d_reg, 0, d_identity, NM, nc};
+    out = SegSrc{d_off, d_len, d_rows, d_tmin, d_tmax, d_reg, 0, nullptr, NM, nc};
     return OG_OK;
 }
 
@@ -753,11 +768,23 @@ int spliced_totals(const Spliced &sd, uint32_t nc, ShardState &out, const char *
     return OG_OK;
 }
 
-void take_spliced(Scratch &own, Spliced &sd, ShardState &out) {
+int install_state(og_shard *s, og_shard &out, Scratch &own, Spliced &sd, const std::vector<uint32_t> &series_seg_begin,
+                  const std::vector<uint64_t> &sids, const std::vector<int32_t> &types, const std::vector<std::string> &names) {
+    int rc;
+    const size_t n_series = sids.size();
+    out.device = s->device; out.n_series = (uint32_t)n_series; out.n_segments = sd.n; out.n_columns = sd.n_columns;
+    out.sids = sids; out.col_types = types; out.col_names = names; out.h_series_seg_begin = series_seg_begin;
+    if ((rc = dalloc(&out.d_series_seg_begin, n_series + 1)) || (rc = dalloc(&out.d_sids, n_series))) return rc;
+    CU(cudaMemcpy(out.d_series_seg_begin, series_seg_begin.data(), (n_series + 1) * 4, cudaMemcpyHostToDevice));
+    if (n_series) CU(cudaMemcpy(out.d_sids, sids.data(), n_series * 8, cudaMemcpyHostToDevice));
     auto take = [&](void *p) { own.bufs.erase(std::find(own.bufs.begin(), own.bufs.end(), p)); };
     for (void *p : {(void *)sd.off, (void *)sd.len, (void *)sd.rows, (void *)sd.series, (void *)sd.tmin, (void *)sd.tmax, (void *)sd.data}) take(p);
     out.d_page_off = sd.off; out.d_page_len = sd.len; out.d_seg_rows = sd.rows; out.d_seg_series = sd.series; out.d_tmin = sd.tmin; out.d_tmax = sd.tmax;
     out.d_data = sd.data; out.data_len = sd.data_len; out.owns_data = true;
+    CU(cudaDeviceSynchronize());
+    std::swap(static_cast<ShardState &>(*s), static_cast<ShardState &>(out));
+    s->reset_il();
+    return OG_OK;
 }
 
 /* ---------------------------------------------------------------- files into a shard */
@@ -782,9 +809,8 @@ int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flag
     std::vector<uint64_t> sids;
     for (auto &kv : series_of_sid) { kv.second = (uint32_t)sids.size(); sids.push_back(kv.first); }
     const uint32_t nc = (uint32_t)names.size(), NSER = (uint32_t)sids.size();
-    std::vector<int32_t> col_of_old(nc, -1), identity(nc);
+    std::vector<int32_t> col_of_old(nc, -1);
     for (uint32_t c = 0; c < onc; c++) col_of_old[std::lower_bound(names.begin(), names.end(), s->col_names[c]) - names.begin()] = (int32_t)c;
-    for (uint32_t c = 0; c < nc; c++) identity[c] = (int32_t)c;
     std::vector<int64_t> old_of(NSER, -1);
     for (auto &kv : old_of_sid) old_of[series_of_sid[kv.first]] = kv.second;
     /* ---- the new files' directory; per series their ordered segments (file order) and out-of-order segments ---- */
@@ -803,33 +829,18 @@ int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flag
             probe_u.push_back(u); probe_old.push_back((uint32_t)old_of[u]); probe_lo.push_back(span_lo[u]); probe_hi.push_back(span_hi[u]);
         }
     }
-    const uint32_t NP = (uint32_t)probe_u.size();
     std::vector<uint32_t> old_a(NSER, 0), old_b(NSER, 0);
-    {
-        Scratch t;
-        uint32_t *d_ser, *d_a, *d_b; int64_t *d_lo, *d_hi, *d_last;
-        if ((rc = t.get(&d_ser, NP)) || (rc = t.get(&d_lo, NP)) || (rc = t.get(&d_hi, NP)) || (rc = t.get(&d_last, NP)) || (rc = t.get(&d_a, NP)) || (rc = t.get(&d_b, NP))) return rc;
-        if (NP) {
-            CU(cudaMemcpy(d_ser, probe_old.data(), NP * 4ull, cudaMemcpyHostToDevice));
-            CU(cudaMemcpy(d_lo, probe_lo.data(), NP * 8ull, cudaMemcpyHostToDevice));
-            CU(cudaMemcpy(d_hi, probe_hi.data(), NP * 8ull, cudaMemcpyHostToDevice));
-            k_append_probe<<<(NP + 127) / 128, 128>>>(s->d_series_seg_begin, s->d_tmin, s->d_tmax, d_ser, d_lo, d_hi, NP, d_last, d_a, d_b);
-            CU(cudaGetLastError());
-            std::vector<int64_t> last(NP); std::vector<uint32_t> a(NP), b(NP);
-            CU(cudaMemcpy(last.data(), d_last, NP * 8ull, cudaMemcpyDeviceToHost));
-            CU(cudaMemcpy(a.data(), d_a, NP * 4ull, cudaMemcpyDeviceToHost));
-            CU(cudaMemcpy(b.data(), d_b, NP * 4ull, cudaMemcpyDeviceToHost));
-            for (uint32_t k = 0; k < NP; k++) {
-                const uint32_t u = probe_u[k];
-                /* the flush rule: a series' new ordered rows start after the last time the shard holds for it */
-                if (!ordered[u].empty() && fd.tmin[ordered[u][0]] <= last[k]) {
-                    set_error("series sid %llu: ordered file %u starts at %lld, not after the shard's last time %lld; only out-of-order files may overlap the shard",
-                              (unsigned long long)sids[u], fd.src_file[ordered[u][0]], (long long)fd.tmin[ordered[u][0]], (long long)last[k]);
-                    return OG_E_UNSUPPORTED;
-                }
-                old_a[u] = a[k]; old_b[u] = b[k];
-            }
+    Probe pr;
+    if ((rc = probe_series(s, probe_old, probe_lo.data(), probe_hi.data(), pr))) return rc;
+    for (size_t k = 0; k < probe_u.size(); k++) {
+        const uint32_t u = probe_u[k];
+        /* the flush rule: a series' new ordered rows start after the last time the shard holds for it */
+        if (!ordered[u].empty() && fd.tmin[ordered[u][0]] <= pr.last[k]) {
+            set_error("series sid %llu: ordered file %u starts at %lld, not after the shard's last time %lld; only out-of-order files may overlap the shard",
+                      (unsigned long long)sids[u], fd.src_file[ordered[u][0]], (long long)fd.tmin[ordered[u][0]], (long long)pr.last[k]);
+            return OG_E_UNSUPPORTED;
         }
+        old_a[u] = pr.a[k]; old_b[u] = pr.b[k];
     }
     /* ---- layout: per series the shard's segments then its new ordered ones (one time-ordered list of n_old + n_new); a span
        rewrites the list's [before, after_begin) with the out-of-order segments ---- */
@@ -856,25 +867,16 @@ int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flag
     if ((rc = dev ? place_files(files, n_files, names, types, s->device, fd, *dev, nw, new_rows)
                   : upload_files(files, n_files, names, types, s->device, fd, nw, new_rows)))
         return rc;
-    /* the interleaved copies describe the old layout: dropped now, rebuilt by the first query that wants them */
-    {
-        std::lock_guard<std::mutex> il_lock(s->il_mu);
-        for (og_shard::IlCol &c : s->il)
-            dev_free_all(c.words, c.grp_off, c.grp_rows, c.grp_col, c.lane_seg, c.lane_rows, c.lane_series, c.lane_win, c.lane_t0, c.lane_dt, c.gen_list);
-        s->il.assign(s->n_columns, og_shard::IlCol{});
-    }
+    s->reset_il(); /* the copies describe the old layout: their memory serves the pass */
     Scratch d_maps;
-    int32_t *d_col_old, *d_identity;
-    if ((rc = d_maps.get(&d_col_old, nc)) || (rc = d_maps.get(&d_identity, nc))) return rc;
+    int32_t *d_col_old;
+    if ((rc = d_maps.get(&d_col_old, nc))) return rc;
     CU(cudaMemcpy(d_col_old, col_of_old.data(), nc * 4ull, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(d_identity, identity.data(), nc * 4ull, cudaMemcpyHostToDevice));
     SegSrc src[3] = {};
     src[SRC_SHARD] = SegSrc{s->d_page_off, s->d_page_len, s->d_seg_rows, s->d_tmin, s->d_tmax, nullptr, 0, d_col_old, ONSEG, onc};
-    src[SRC_FILES] = SegSrc{nw->d_page_off, nw->d_page_len, nw->d_seg_rows, nw->d_tmin, nw->d_tmax, nullptr, 1, d_identity, NN, nc};
-    cudaEvent_t ev0, ev1;
-    CU(cudaEventCreate(&ev0)); CU(cudaEventCreate(&ev1));
-    struct FreeEv { cudaEvent_t a, b; ~FreeEv() { cudaEventDestroy(a); cudaEventDestroy(b); } } free_ev{ev0, ev1};
-    CU(cudaEventRecord(ev0, 0));
+    src[SRC_FILES] = SegSrc{nw->d_page_off, nw->d_page_len, nw->d_seg_rows, nw->d_tmin, nw->d_tmax, nullptr, 1, nullptr, NN, nc};
+    EventTimer timer;
+    CU(timer.start());
     /* ---- merge: the spans' source segments spliced into one directory (the shard's rows first, then the new files in sequence,
        ordered before out-of-order), then merge_spans ---- */
     std::vector<NewSegs> batches;
@@ -923,7 +925,7 @@ int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flag
     std::vector<uint32_t> m_first;
     std::vector<const uint8_t *> regions = {s->d_data, nw->d_data};
     Scratch m_own;
-    if ((rc = batches_source(batches, nc, d_identity, 2, regions, m_own, src[SRC_MERGED], m_first))) return rc;
+    if ((rc = batches_source(batches, nc, 2, regions, m_own, src[SRC_MERGED], m_first))) return rc;
     /* ---- the new directory as runs: per series the shard's segments before its span, new ordered ones before it, the span's
        merged segments, then the rest of both ---- */
     std::vector<Run> runs;
@@ -953,7 +955,7 @@ int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flag
     Spliced sd;
     if ((rc = splice_and_gather(src, runs, NOUT, nc, regions, out_own, sd))) return rc;
     if (!sd.data) { sd.data = nw->d_data; sd.data_len = nw->data_len; nw->d_data = nullptr; out_own.bufs.push_back(sd.data); }
-    CU(cudaEventRecord(ev1, 0));
+    CU(timer.stop());
     /* ---- derived state ---- */
     if ((rc = spliced_totals(sd, nc, *out, "the append"))) return rc;
     /* the Snappy counters hold while every transcoded page is in the shard: the first merge drops them */
@@ -963,26 +965,29 @@ int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flag
         out->snappy_bytes_in = s->snappy_bytes_in + nw->snappy_bytes_in; out->snappy_bytes_out = s->snappy_bytes_out + nw->snappy_bytes_out;
     }
     out->page_bytes = out->page_bytes - out->snappy_bytes_out + out->snappy_bytes_in;
-    /* ---- the new state, complete and synchronised before it is swapped in: nothing fails after the swap ---- */
-    out->device = s->device; out->n_series = NSER; out->n_segments = NOUT; out->n_columns = nc;
-    out->sids = sids; out->col_types = types; out->col_names = names; out->h_series_seg_begin = o_ssb;
-    if ((rc = dalloc(&out->d_series_seg_begin, (size_t)NSER + 1)) || (rc = dalloc(&out->d_sids, (size_t)NSER))) return rc;
-    CU(cudaMemcpy(out->d_series_seg_begin, o_ssb.data(), ((size_t)NSER + 1) * 4, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(out->d_sids, sids.data(), (size_t)NSER * 8, cudaMemcpyHostToDevice));
-    float ms = 0;
-    CU(cudaEventElapsedTime(&ms, ev0, ev1));
-    info.merge_ms = ms;
+    CU(timer.ms(&info.merge_ms));
     info.rows_after_merge = out->n_rows;
-    take_spliced(out_own, sd, *out);
     out->merge = info;
-    CU(cudaDeviceSynchronize());
-    /* swap the whole state: `out` takes the old one and frees it on return (the caller's buffer of a shard opened in place is not
-       freed) */
-    std::swap(static_cast<ShardState &>(*s), static_cast<ShardState &>(*out));
-    {
-        std::lock_guard<std::mutex> il_lock(s->il_mu);
-        s->il.assign(s->n_columns, og_shard::IlCol{});
-    }
+    return install_state(s, *out, out_own, sd, o_ssb, sids, types, names);
+}
+
+/* ---------------------------------------------------------------- the entry points that rewrite a shard or open one */
+
+int rewrite_shard(og_shard *s, const char *verb, const std::function<int()> &pass) {
+    std::lock_guard<std::mutex> lock(s->live->mu); /* og_query_create waits until the rewrite is done */
+    if (s->live->n) { set_error("%u queries on this shard are still open: destroy them before %s", s->live->n, verb); return OG_E_STATE; }
+    CU(cudaSetDevice(s->device));
+    return pass();
+}
+
+int open_empty(og_shard **out, const std::function<int(og_shard *)> &pass) {
+    *out = nullptr;
+    int rc = ensure_device(); if (rc) return rc;
+    std::unique_ptr<og_shard> s(new og_shard);
+    CU(cudaGetDevice(&s->device));
+    s->h_series_seg_begin = {0};
+    if ((rc = pass(s.get()))) return rc;
+    *out = s.release();
     return OG_OK;
 }
 
@@ -994,22 +999,12 @@ extern "C" {
 
 OG_API int og_shard_open_files(const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, og_shard **out) {
     if (!files || !out || n_files == 0) { set_error("null argument or no files"); return OG_E_INVAL; }
-    *out = nullptr;
-    int rc = ensure_device(); if (rc) return rc;
-    std::unique_ptr<og_shard> s(new og_shard); /* an open is an append to an empty shard */
-    CU(cudaGetDevice(&s->device));
-    s->h_series_seg_begin = {0};
-    if ((rc = add_files(s.get(), files, file_flags, n_files, "og_shard_open_files", nullptr))) return rc;
-    *out = s.release();
-    return OG_OK;
+    return open_empty(out, [&](og_shard *s) { return add_files(s, files, file_flags, n_files, "og_shard_open_files", nullptr); });
 }
 
 OG_API int og_shard_append_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files) {
     if (!s || !files || n_files == 0) { set_error("null argument or no files"); return OG_E_INVAL; }
-    std::lock_guard<std::mutex> lock(s->live->mu); /* og_query_create waits until the append is done */
-    if (s->live->n) { set_error("%u queries on this shard are still open: destroy them before appending files", s->live->n); return OG_E_STATE; }
-    CU(cudaSetDevice(s->device));
-    return add_files(s, files, file_flags, n_files, "og_shard_append_files", nullptr);
+    return rewrite_shard(s, "appending files", [&] { return add_files(s, files, file_flags, n_files, "og_shard_append_files", nullptr); });
 }
 
 OG_API int og_shard_merge_info(const og_shard *s, og_merge_info *out) {

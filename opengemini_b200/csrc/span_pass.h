@@ -6,6 +6,7 @@
  */
 #pragma once
 #include <cstdint>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -28,7 +29,8 @@ enum { SRC_SHARD = 0, SRC_FILES = 1, SRC_MERGED = 2 };
 /* consecutive output segments [out0, next run's out0) of one series, from consecutive segments src0... of source `kind` */
 struct Run { uint32_t out0, src0, series, kind; };
 
-/* one source of spliced segments: a device directory whose column c is column col[c] of the source (-1: the source lacks it) */
+/* one source of spliced segments: a device directory whose column c is column col[c] of the source (-1: the source lacks it), or
+ * column c itself when col is null */
 struct SegSrc {
     const uint64_t *off; const uint32_t *len, *rows; const int64_t *tmin, *tmax;
     const uint32_t *seg_region; uint32_t region; /* data region of segment i: seg_region[i], or `region` when seg_region is null */
@@ -59,9 +61,11 @@ int batch_cap_rows(uint64_t per_row, uint64_t floor_rows, const char *env, uint6
  * place relative to the blob, *used grows by the bytes written */
 int encode_columns(const std::vector<int32_t> &types, const int64_t *d_times, const std::vector<uint8_t *> &d_cols, const uint8_t *d_ok,
                    size_t out_rows, const uint32_t *d_rows, uint32_t n, uint32_t rps, uint8_t *blob, uint64_t cap, NewSegs &ns, uint64_t *used);
-/* the first `used` bytes of a batch's scratch blob kept in a buffer of `blobs` followed by 1024 zero bytes (k_append_gather reads
- * past a page's end) */
-int keep_blob(const uint8_t *blob, uint64_t used, Scratch &blobs, NewSegs &ns);
+/* the end of a batch of ns.n new segments: their time ranges read back from d_tmin / d_tmax, their rows, and the first `used`
+ * bytes of the batch's scratch blob kept in a buffer of `blobs` followed by 1024 zero bytes (k_append_gather reads past a page's
+ * end), so the batch's scratch can go back to the pool before the next batch */
+int keep_blob(const int64_t *d_tmin, const int64_t *d_tmax, std::vector<uint32_t> rows, const uint8_t *blob, uint64_t used, Scratch &blobs,
+              NewSegs &ns);
 
 #define MERGE_RPS 1000u /* rows per rewritten segment: lib/util/util.go:72 */
 
@@ -89,9 +93,15 @@ int find_runs(SortedRows &r, const uint32_t *row_file, Scratch &b, MergeErr *d_e
 int combine_and_encode(const SortedRows &r, const std::vector<int32_t> &types, const int32_t *d_types, Scratch &b, unsigned long long *d_rep,
                        uint8_t *span_has, Scratch &blobs, NewSegs &ns, std::vector<uint32_t> &seg_first);
 
-/* per probed series: its last time, and the range [a, b) of its segments that a span [lo, hi] overlaps (merge.cu) */
-__global__ void k_append_probe(const uint32_t *series_seg_begin, const int64_t *seg_tmin, const int64_t *seg_tmax, const uint32_t *series,
-                               const int64_t *lo, const int64_t *hi, uint32_t n, int64_t *last, uint32_t *a_out, uint32_t *b_out);
+/* per series series[k] of `s`: last[k] its last time (INT64_MIN when it holds no segment) and, when `lo` / `hi` are given ([n]
+ * each), [a[k], b[k]) the range of its segments that [lo[k], hi[k]] overlaps */
+struct Probe { std::vector<int64_t> last; std::vector<uint32_t> a, b; };
+int probe_series(const og_shard *s, const std::vector<uint32_t> &series, const int64_t *lo, const int64_t *hi, Probe &out);
+
+/* pages from regions[page_region[p]] + src_off[p] to out + dst_off[p] (len[p] bytes each) with k_append_gather: the flush's
+ * pages into the region of its files (flush.cu) */
+int gather_pages(const std::vector<const uint8_t *> &regions, const std::vector<uint32_t> &page_region, const std::vector<uint64_t> &src_off,
+                 const std::vector<uint32_t> &len, const std::vector<uint64_t> &dst_off, uint8_t *out);
 
 /* New files whose pages are already on the device, as the flush (flush.cu) produces them: file f's pages at data + base[f], where
  * build_file_dir places a file set (16-byte aligned, back to back), followed by 1024 zero bytes; rows[] the rows of every segment,
@@ -109,14 +119,22 @@ struct DeviceFiles {
  * files' pages are on the device already (files[f].data is then never read) */
 int add_files(og_shard *s, const og_shard_desc *files, const uint32_t *file_flags, uint32_t n_files, const char *who, DeviceFiles *dev);
 
+/* The entry points that rewrite an open shard (og_shard_append_files, og_shard_append_rows, og_shard_compact): `pass` runs on the
+ * shard's device under its live-query lock, so og_query_create waits until it is done; while a query lives the call is refused
+ * with OG_E_STATE ("... destroy them before <verb>"). */
+int rewrite_shard(og_shard *s, const char *verb, const std::function<int()> &pass);
+/* The entry points that open a shard by a pass over an empty one (og_shard_open_files, og_shard_open_rows): the shard is created
+ * on the library's device, `pass` runs on it, and it goes to *out when the pass succeeds */
+int open_empty(og_shard **out, const std::function<int(og_shard *)> &pass);
+
 /* the refusal of a string value inside a span `pass` re-encodes, or of a page that failed to decode in segment `seg` of `where` */
 int string_refusal(unsigned long long sid, const std::string &column, const char *pass);
 int decode_failure(int device_code, uint32_t seg, const char *where);
 
-/* the new segments of every batch as one source directory (SRC_MERGED); batch b's blob is region first_region + b, appended to
- * `regions`.  m_first[b] is the first segment of batch b in it. */
-int batches_source(const std::vector<NewSegs> &batches, uint32_t n_columns, const int32_t *d_identity, uint32_t first_region,
-                   std::vector<const uint8_t *> &regions, Scratch &own, SegSrc &out, std::vector<uint32_t> &m_first);
+/* the new segments of every batch as one source directory (SRC_MERGED) over the pass's columns; batch b's blob is region
+ * first_region + b, appended to `regions`.  m_first[b] is the first segment of batch b in it. */
+int batches_source(const std::vector<NewSegs> &batches, uint32_t n_columns, uint32_t first_region, std::vector<const uint8_t *> &regions,
+                   Scratch &own, SegSrc &out, std::vector<uint32_t> &m_first);
 
 /* k_append_splice over `runs`, then the referenced pages gathered into one new buffer unless every run reads the files' region */
 int splice_and_gather(const SegSrc src[3], const std::vector<Run> &runs, uint32_t n_out, uint32_t n_columns,
@@ -125,7 +143,12 @@ int splice_and_gather(const SegSrc src[3], const std::vector<Run> &runs, uint32_
 /* n_rows, page_bytes, irregular_time_pages, max_seg_rows, tmin / tmax of a spliced directory (k_append_stats) into `out` */
 int spliced_totals(const Spliced &sd, uint32_t n_columns, ShardState &out, const char *who);
 
-/* the directory arrays and data region of `sd` handed from `own` to `out` */
-void take_spliced(Scratch &own, Spliced &sd, ShardState &out);
+/* The new state `out`, built apart, becomes s's.  The caller has run spliced_totals into `out` and set the fields its pass owns
+ * (merge info, rows_merged, Snappy counters).  This completes the header from the series begin list, sids, column types and
+ * names, uploads d_series_seg_begin and d_sids, hands sd's directory arrays and data region from `own` to `out`, synchronises,
+ * swaps, and drops s's interleaved copies.  Nothing fails after the swap; on an earlier error `s` is as it was.  `out` leaves with
+ * the old state, which it frees when the caller drops it (the caller's buffer of a shard opened in place is not freed). */
+int install_state(og_shard *s, og_shard &out, Scratch &own, Spliced &sd, const std::vector<uint32_t> &series_seg_begin,
+                  const std::vector<uint64_t> &sids, const std::vector<int32_t> &types, const std::vector<std::string> &names);
 
 } // namespace ogpu

@@ -229,8 +229,6 @@ __global__ void k_tssp_crc_fold(WriteP w, const uint64_t *slot_off, const uint32
     p[0] = (uint8_t)(crc >> 24); p[1] = (uint8_t)(crc >> 16); p[2] = (uint8_t)(crc >> 8); p[3] = (uint8_t)crc;
 }
 
-double ms_since(std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
-
 } // namespace
 
 struct og_tssp_image {
@@ -291,7 +289,7 @@ OG_API int og_shard_write_tssp(og_shard *s, const og_tssp_write_desc *d, og_tssp
     CU(cudaMemcpy(err, d_err, 8, cudaMemcpyDeviceToHost));
     if (err[0]) {
         set_error("segment %d failed to decode (device code %d)", err[1], err[0]);
-        return err[0] == D_UNSUPPORTED ? OG_E_UNSUPPORTED : err[0] == D_TYPE ? OG_E_TYPE : OG_E_CORRUPT;
+        return map_dev_err(err[0]);
     }
     img->phase_ms[0] = ms_since(t0);
 

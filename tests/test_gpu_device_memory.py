@@ -14,6 +14,7 @@ import torch
 import oracle
 from opengemini_b200 import AggQuery, Shard, write_tssp
 from opengemini_b200 import _lib as L
+from test_gpu_out_of_order import _file_desc, _series
 
 pytestmark = pytest.mark.gpu
 T0, SEC = 1_700_000_000_000_000_000, 1_000_000_000
@@ -145,6 +146,51 @@ def test_open_files_releases_the_file_set(out_of_order):
         assert (sh.merge_info()["series_merged"] > 0) == out_of_order
         q = AggQuery(sh, [("sum", 0), ("count", 0)], 60 * SEC, T0, T0 + 3000 * SEC).run()
         q.close()
+        sh.close()
+
+
+def test_append_flush_and_compaction_release_what_they_replace():
+    """One shard through every rewrite, each after a query that built the lane-interleaved copy of the layout it replaces, and each
+    refused once on the way: the copies, the old state and the passes' scratch all go back to the pool."""
+    n = 3000
+    t = T0 + np.arange(n, dtype=np.int64) * SEC
+    ok = np.ones(n, bool)
+    rng = np.random.default_rng(12)
+    # sid 1 holds string values in full segments: a re-cut at 700 rows reaches them, one at 1000 rows leaves the series alone
+    base = {1: _series(t, {"v": (L.TYPE_FLOAT, 100 + rng.random(n), ok), "s": (TYPE_STRING, None, ok)}),
+            2: _series(t, {"v": (L.TYPE_FLOAT, 100 + rng.random(n), ok)})}
+    late_t = T0 + np.arange(500, 900, dtype=np.int64) * SEC + SEC // 2
+    late = {2: _series(late_t, {"v": (L.TYPE_FLOAT, 100 + rng.random(late_t.size), np.ones(late_t.size, bool))})}
+    rows_t = np.concatenate([T0 + np.arange(1000, 1100, dtype=np.int64) * SEC + SEC // 4, T0 + np.arange(n, n + 700, dtype=np.int64) * SEC])
+    rows = {2: _series(rows_t, {"v": (L.TYPE_FLOAT, 100 + rng.random(rows_t.size), np.ones(rows_t.size, bool))})}
+
+    def query(sh):
+        q = AggQuery(sh, [("sum", 1), ("count", 1)], 60 * SEC, T0, T0 + (n + 700) * SEC).run()
+        assert q.stats()["il_state"] == 1
+        return q
+
+    def refused(status, text, call):
+        with pytest.raises(L.OgpuError) as ei:
+            call()
+        assert ei.value.status == status and text in str(ei.value), str(ei.value)
+
+    with _NoLeak():
+        sh = Shard.open_files([(_file_desc(base), False)])
+        q = query(sh)
+        refused(L.OG_E_STATE, "before appending files", lambda: sh.append_files([(_file_desc(late), True)]))
+        q.close()
+        sh.append_files([(_file_desc(late), True)])
+        assert sh.merge_info()["series_merged"] == 1
+        q = query(sh)
+        refused(L.OG_E_STATE, "before appending rows", lambda: sh.append_rows(rows))
+        q.close()
+        assert sh.append_rows(rows)["out_of_order_rows"] == 100
+        q = query(sh)
+        refused(L.OG_E_STATE, "before compacting it", lambda: sh.compact())
+        q.close()
+        refused(L.OG_E_UNSUPPORTED, "string column", lambda: sh.compact(700))
+        assert sh.compact()["series_rewritten"] == 1
+        query(sh).close()
         sh.close()
 
 
